@@ -1,8 +1,9 @@
-"""Benchmark of the NeRO stage-I training hot path on B200 (BASELINE.json metric: train rays/sec at 128 samples/ray).
+"""Benchmark of the NeRO stage-I training hot path on H100 (BASELINE.json metric: train rays/sec at 128 samples/ray).
 
     python bench.py --gpus 1 --steps 20 --warmup 5                 # this repo's CUDA path
     torchrun ... bench.py --gpus N ...                             # ray-sharded data parallel, one rank per GPU
     python bench.py --impl reference ...                           # the reference algorithm (oracle port) on the host CPU
+    python bench.py ... --dump-outputs DIR                          # also write the last timed step's results as DIR/*.npy
 
 A "step" = one training step on the workload of BASELINE.json configs[1] ("bell shape stage, 1024 rays x 128 samples"):
 sample_ray (64 coarse + 4x16 up-sampled + 32 background samples) + render_core forward + the YAML loss set
@@ -16,7 +17,8 @@ Three legs, all on THE SAME 1024 synthetic rays per GPU (nero_b200.synthetic.syn
           `e2e.train_ray_num_512`;
   bear    the same resident loop on BASELINE.json configs[2] (human light, 2048 rays on one GPU; 1024 per GPU under
           torchrun = configs[4] at 8 GPUs), reported under the key "bear" of the same JSON line.
-Prints ONE JSON line (see the driver contract in the task statement).
+Every leg times --steps steps.  Inputs are seeded: the same arguments give the same inputs on every run, so --dump-outputs of
+two builds can be compared output for output.  Prints ONE JSON line.
 """
 import argparse
 import json
@@ -47,7 +49,7 @@ def workload_config(bear, R, world):
             f'bell_shape_stage_{R}rays_x_(64+64)samples_+32bg_step30000_occ_on')
     return {'workload': name, 'rays_per_gpu': R, 'global_rays': R * world,
             'parallelism': f'ray-sharded dp{world}, one NCCL all-reduce of the flat grad buffer' if world > 1 else 'single gpu',
-            'l2': 'per-step working set ~6 GB of activations >> 126 MB L2 (inputs larger than L2)',
+            'l2': 'per-step working set ~6 GB of activations >> 50 MB L2 (inputs larger than L2)',
             'optimizer': 'Adam inside the timed region'}
 
 
@@ -67,8 +69,9 @@ def measured_peaks():
     path = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     if os.path.exists(path):
         d = json.load(open(path))
-        return d.get('bf16_tflops_sustained', 1386.8), d.get('hbm_gbs', 6569.6), 'measured'
-    return 1400.0, 6650.0, 'fallback'
+        return d.get('bf16_tflops_sustained', 989.4), d.get('hbm_gbs', 3350.0), 'measured'
+    # NVIDIA H100 SXM data sheet (dense BF16, HBM3) for a 700 W card; a card set to a lower power limit reaches less
+    return 989.4, 3350.0, 'H100 SXM data sheet'
 
 
 class ClockSampler(threading.Thread):
@@ -182,7 +185,23 @@ class Workload:
         loss.backward()
         self.sync_grads()
         self.opt.step()
+        self.last = (z, out, loss)
         return loss
+
+    def dump_outputs(self, d):
+        """What the last resident step handed its caller -- z_vals, every render_core output, the loss -- plus the parameter
+        gradients of that step and the parameters after its Adam update, as float32 / float64 .npy files (about 20 MB)."""
+        os.makedirs(d, exist_ok=True)
+        z, out, loss = self.last
+        arrays = {'z_vals': z, 'loss': loss.reshape(1)}
+        arrays.update({f'out.{k}': v for k, v in out.items() if torch.is_tensor(v)})
+        for n, p in self.net.named_parameters():
+            if p.grad is not None:
+                arrays[f'grad.{n}'] = p.grad
+            arrays[f'param.{n}'] = p
+        for k, v in arrays.items():
+            v = v.detach().cpu()
+            np.save(os.path.join(d, k + '.npy'), v.numpy() if v.dtype == torch.float64 else v.float().numpy())
 
     def e2e_step(self, step):
         self.opt.zero_grad(set_to_none=True)
@@ -254,6 +273,8 @@ def run_ours(args):
     l0 = ops.launch_count
     ms = timed(lambda i: wl.resident_step(), args.steps, barrier)
     launches = (ops.launch_count - l0) // args.steps
+    if args.dump_outputs and rank == 0:
+        wl.dump_outputs(args.dump_outputs)
     n_in, n_out, p_occ = wl.counts()
 
     # ---- end to end through the public API with host buffers (H2D of the ray batch + D2H of the loss every step):
@@ -289,7 +310,7 @@ def run_ours(args):
         wb = Workload(True, rank, world, dev)
         for _ in range(3):
             wb.resident_step()
-        ksteps = max(3, min(args.steps, 10))
+        ksteps = args.steps
         ms_b = timed(lambda i: wb.resident_step(), ksteps, barrier)
         nb_in, nb_out, pb = wb.counts()
         ms_b, = reduce_max([ms_b])
@@ -325,22 +346,15 @@ def run_ours(args):
             one = prof['reverse_sweep']
             ach_tf = one['flops'] / one['seconds'] / 1e12
             # algorithmic HBM bytes of the launch: the first operand in + 8 layers x (saved activation in + product out), 1 KB per
-            # row and tensor (DESIGN.md section 4); the decoupling experiments of profiles/r02j show the kernel nearer to this roof
-            # (epilogue + operand traffic alone: 82 % of the coupled time) than to the tensor roof (MMAs alone: 49 %)
+            # row and tensor (DESIGN.md section 4)
             alg_bytes = one['rows'] * 17408.0
             ach_bw = alg_bytes / one['seconds'] / 1e9
-            traffic, tsrc = None, None
-            tp = os.path.join(ROOT, 'profiles', 'chain_traffic.json')
-            if os.path.exists(tp):      # ncu dram__bytes_read+write of this launch, recorded per row; scaled to this run's rows
-                tj = json.load(open(tp))
-                traffic, tsrc = tj['dram_bytes_per_row'] * one['rows'], tj.get('source')
-            line['roofline'] = {'bound': 'hbm', 'kernel': 'umma_chain_kernel: SDF reverse-sweep chain (8 fused 256-wide layers, one launch)',
+            line['roofline'] = {'bound': 'hbm', 'kernel': 'gemm_chain_kernel: SDF reverse-sweep chain (8 fused 256-wide layers, one launch)',
                                 'achieved': ach_bw, 'peak': peak_bw, 'unit': 'GB/s', 'frac': ach_bw / peak_bw,
-                                'peak_source': which + ' HBM copy bandwidth', 'algorithmic_bytes': alg_bytes,
-                                'launch_us': one['seconds'] * 1e6, 'rows': one['rows'], 'traffic': traffic, 'traffic_source': tsrc,
-                                'traffic_frac_of_peak': None if traffic is None else traffic / one['seconds'] / 1e9 / peak_bw,
+                                'peak_source': which + ' HBM bandwidth', 'algorithmic_bytes': alg_bytes,
+                                'launch_us': one['seconds'] * 1e6, 'rows': one['rows'],
                                 'tensor': {'achieved': ach_tf, 'peak': peak_tf, 'unit': 'TFLOP/s', 'frac': ach_tf / peak_tf,
-                                           'frac_of_split3_ceiling': ach_tf / (peak_tf / 3.0), 'peak_source': which + ' bf16 sustained',
+                                           'frac_of_split3_ceiling': ach_tf / (peak_tf / 3.0), 'peak_source': which + ' bf16',
                                            'note': 'ALGORITHMIC fp32 GEMM flops (2*M*K*N of the un-padded layers); the split-bf16 scheme '
                                                    'issues 3 bf16 MMAs per product, so 1/3 of peak is its ceiling'},
                                 'all_chain_launches': {'launches': prof['launches'], 'total_ms': prof['seconds'] * 1e3,
@@ -357,8 +371,7 @@ def run_ours(args):
 
 def profile_chains(wl):
     """One extra training step with a CUDA-event pair (on the launch stream) around every fused MLP-chain launch
-    (ops.PROFILE hook).  Returns the aggregate over all chain launches and the SDF reverse-sweep chain alone (the
-    launch whose ncu capture is committed under profiles/)."""
+    (ops.PROFILE hook).  Returns the aggregate over all chain launches and the SDF reverse-sweep chain alone."""
     from nero_b200 import ops
     net, r = wl.net, wl.r
     ops.PROFILE = []
@@ -493,6 +506,9 @@ def main():
                     help="bell = BASELINE.json configs[1] (the headline, default); bear = configs[2]: human light, 2048 rays")
     ap.add_argument('--no-cpu', action='store_true', help='skip the cpu_baseline leg (profiling runs)')
     ap.add_argument('--no-bear', action='store_true', help='skip the second workload (configs[2]) record')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write what the last timed step computed (z_vals, render outputs, loss, gradients, updated parameters) '
+                         'as DIR/<name>.npy')
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     if args.impl == 'reference':

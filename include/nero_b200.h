@@ -1,4 +1,4 @@
-/* libnero_b200 -- C ABI of the B200-native NeRO stage-I volume-rendering hot path.
+/* libnero_b200 -- C ABI of the H100-native (sm_90a) NeRO stage-I volume-rendering hot path.
  *
  * There is no FFI in the reference (it is pure PyTorch); the boundary this library sits behind is the Python
  * nn.Module contract of network/renderer.py (NeROShapeRenderer.render / render_core) -- see INTEGRATION.md.
@@ -39,7 +39,7 @@ int nero_prep_weight(const float* v, const float* g, int K, int row0, int nrows,
                      void* img_f, int rows_pad_f, void* img_t, int rows_pad_t, int t_c0, int t_ncols, float* w_eff, int ld_weff,
                      void* stream);
 
-/* ---- fused linear layer on tcgen05 tensor cores ----------------------------------------------------------
+/* ---- fused linear layer on wgmma tensor cores ------------------------------------------------------------
  * out = epilogue(A[M,K] * W^T).  Replaces nn.Linear + activation of SDFNetwork.forward (field.py:130-147),
  * NeRFNetwork.forward (field.py:258-283), make_predictor (field.py:310-346) and the autograd input-gradient /
  * double-backward GEMMs of SDFNetwork.gradient (field.py:155-167).
@@ -52,7 +52,7 @@ int nero_linear(const float* A, int lda, int k_valid, const void* wimg, int n_pa
                 const float* addend, int ldadd, int ncol_main, float* tail, int ldt,
                 const int* m_ptr, int m_cap, void* stream);
 
-/* ---- fused MLP chain on tcgen05 (A operand kept in TMEM across layers) ------------------------------------------
+/* ---- fused MLP chain on wgmma (A operand kept in shared memory across layers) -----------------------------------
  * Runs up to 10 consecutive layers of SDFNetwork / make_predictor / NeRFNetwork (network/field.py:130-147, 310-346,
  * 258-283) or of their gradient sweeps on each 128-row tile without writing the inter-layer activations' A operand
  * to HBM.  `chain_params_host` points to a HOST struct nero_chain_params (layout below, natural alignment). */
@@ -76,10 +76,10 @@ int nero_chain(const void* chain_params_host, void* stream);
 int nero_row_axpy(const float* a, int lda, const float* X, int ldx, float* Y, int ldy, int ncol, const int* m_ptr, int m_cap, void* stream);
 
 /* ---- weight gradients -------------------------------------------------------------------------------------
- * partial += dY^T X (+ dY2^T X2): P CTAs per 128-row output tile each contract a slice of the sample rows and ADD their tile
- * into the one [rows_partial x ld_partial] fp32 accumulator `partial` (and the column sums of dY into `bias_partial`
- * [rows_partial]) with L2 reductions; the caller zeroes both before the call.  Replaces the autograd weight-gradient GEMMs;
- * nero_wgrad_finish is then called with P = 1. */
+ * partial += dY^T X (+ dY2^T X2): P CTAs per 128-row output tile each contract a slice of the sample rows and add their tile
+ * into their own slice p of the [P x rows_partial x ld_partial] fp32 accumulator `partial` (and the column sums of dY into
+ * `bias_partial` [P x rows_partial]); the caller zeroes both before the call.  No atomics: the result is the same every run.
+ * Replaces the autograd weight-gradient GEMMs; nero_wgrad_finish is then called with the same P. */
 int nero_wgrad(const float* dY, int ldy, int n_valid, const float* X, int ldx, int k_valid,
                const float* dY2, int ldy2, const float* X2, int ldx2,
                float* partial, int ld_partial, int rows_partial, float* bias_partial,

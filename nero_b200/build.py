@@ -1,4 +1,4 @@
-"""Build libnero_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Build libnero_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU)."""
 import glob
 import os
 import subprocess
@@ -8,7 +8,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libnero_b200.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC',
+ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
+FLAGS = ARCH + ['-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC',
          '--expt-relaxed-constexpr', '-Xptxas', '-v' if os.environ.get('NERO_PTXAS_V') else '-O3']
 
 
@@ -44,7 +45,7 @@ def build(force=False, verbose=False, extra_flags=(), lib_out=None):
         ok = ok and pr.returncode == 0
     if not ok:
         raise RuntimeError('nvcc failed')
-    cmd = [NVCC, '-shared', '-o', lib_out or LIB] + objs + ['-lcudart']
+    cmd = [NVCC] + ARCH + ['-shared', '-o', lib_out or LIB] + objs + ['-lcudart']
     subprocess.check_call(cmd)
     return lib_out or LIB
 

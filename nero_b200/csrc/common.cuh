@@ -36,7 +36,7 @@
 
 namespace nero {
 
-constexpr int kNumSMs = 148;
+constexpr int kNumSMs = 132;   // H100 SXM
 
 // activation codes shared by the GEMM epilogues and the C ABI
 enum Act : int { ACT_NONE = 0, ACT_SOFTPLUS100 = 1, ACT_RELU = 2, ACT_SIGMOID = 3, ACT_EXPCLAMP = 4 };

@@ -1,0 +1,133 @@
+// Device helpers shared by the wgmma GEMM kernels (k_gemm_linear.cu, k_gemm_chain.cu, k_gemm_wgrad.cu).
+//
+// Every GEMM runs as split-bf16: an fp32 operand x is stored as bf16 hi + bf16 lo (x ~= hi + lo, ~2^-17 relative) and a
+// product is A_lo*B_hi + A_hi*B_lo + A_hi*B_hi (the lo*lo term, ~2^-18 relative, is dropped), accumulated in fp32.
+//
+// Accumulator fragment of wgmma m64nNk16 (fp32): thread t of the warpgroup (warp w = t / 32, lane l) holds d[i] at
+//   row 16 w + l / 4 + 8 ((i / 2) % 2),  column 8 (i / 4) + 2 (l % 4) + (i % 2)
+// i.e. pairs of adjacent columns; the epilogues below work on such pairs.
+#pragma once
+#include "common.cuh"
+#include "ptx.cuh"
+
+namespace nero {
+
+// compile-time epilogue kinds
+enum EpiKind : int { EK_BIAS_SOFTPLUS = 0, EK_BIAS_RELU = 1, EK_BIAS_GENERIC = 2, EK_DACT_SOFTPLUS = 3, EK_DACT_RELU = 4,
+                     EK_DACT_NONE = 5, EK_TANGENT = 6 };
+
+__device__ __forceinline__ float ex2_ftz(float x) {   // MUFU.EX2 without the denormal-range fix-up of exp2f()
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+__device__ __forceinline__ float lg2_ftz(float x) {
+  float y;
+  asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+// fast softplus(beta=100): max error ~1e-9 absolute (ex2/lg2 approximations, 1+t rounding).  softplus(x) >= x everywhere
+// and the clamped branch saturates at softplus(0.2) = 0.2 + 2e-11, so torch's threshold select is a plain max
+__device__ __forceinline__ float softplus100_fast(float x) {
+  const float t = lg2_ftz(1.0f + ex2_ftz(fminf(x, 0.2f) * (100.0f * 1.4426950408889634f)));
+  return fmaxf(x, t * (0.6931471805599453f * 0.01f));
+}
+// sigma(100 a) from h = softplus(a) (possibly stored scaled by 1/hscale): 1 - 2^(-100*log2e*hscale*h); for
+// 100*hscale*h > 20 the exponential is < 2.1e-9, below fp32 resolution of 1 - t, so no branch is needed
+__device__ __forceinline__ float dsoftplus100_fast(float h, float hscale) {
+  return 1.0f - ex2_ftz(-(100.0f * 1.4426950408889634f) * hscale * h);
+}
+
+__device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_t& lo) {
+  __nv_bfloat162 h = __floats2bfloat162_rn(x0, x1);
+  const uint32_t hb = *reinterpret_cast<uint32_t*>(&h);
+  const float h0 = __uint_as_float(hb << 16), h1 = __uint_as_float(hb & 0xffff0000u);
+  __nv_bfloat162 l = __floats2bfloat162_rn(x0 - h0, x1 - h1);
+  hi = hb;
+  lo = *reinterpret_cast<uint32_t*>(&l);
+}
+
+// one 16-deep k-step of the split-bf16 product for one warpgroup (small terms first)
+template <int N, int TA, int TB>
+__device__ __forceinline__ void mma_split3(float* d, uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo, uint32_t acc) {
+  Wgmma<N>::template mma<TA, TB>(d, a_lo, b_hi, acc);
+  Wgmma<N>::template mma<TA, TB>(d, a_hi, b_lo, 1);
+  Wgmma<N>::template mma<TA, TB>(d, a_hi, b_hi, 1);
+}
+
+// two adjacent fp32 values (col, col + 1) of one row; columns >= lim and rows that are not ok read as zero
+__device__ __forceinline__ float2 ld2(const float* __restrict__ g, int ld, long row, int col, int lim, bool ok) {
+  float2 x = make_float2(0.f, 0.f);
+  if (!ok || !g || col >= lim) return x;
+  const float* q = g + row * ld + col;
+  if (col + 1 < lim && (reinterpret_cast<uintptr_t>(q) & 7) == 0) return __ldg(reinterpret_cast<const float2*>(q));
+  x.x = __ldg(q);
+  if (col + 1 < lim) x.y = __ldg(q + 1);
+  return x;
+}
+__device__ __forceinline__ void st2(float* __restrict__ g, int ld, long row, int col, int lim, bool ok, float a, float b) {
+  if (!ok || !g || col >= lim) return;
+  float* q = g + row * ld + col;
+  if (col + 1 < lim && (reinterpret_cast<uintptr_t>(q) & 7) == 0) { *reinterpret_cast<float2*>(q) = make_float2(a, b); return; }
+  q[0] = a;
+  if (col + 1 < lim) q[1] = b;
+}
+
+// operands of the epilogue of one layer (nero_linear / one layer of nero_chain; see include/nero_b200.h)
+struct EpiArgs {
+  const float* bias; int n_bias;
+  float* out; int ldo;
+  const float* H; int ldh; float hscale;
+  const float* addend; int ldadd;
+  const float* V; int ldv;
+  float* out2; int ldo2;
+  float* tail; int ldt;
+  int ncol_out, ncol_main;
+  float oscale; int act; float act_param;
+};
+
+// Epilogue of accumulator columns (col, col + 1) (col even) of one row: writes out / out2 / tail as the kind defines and
+// returns the result values (those a following layer of a chain reads in the main columns).  Rows that are not ok are
+// computed with zero operands and not stored.
+template <int KIND>
+__device__ __forceinline__ float2 epi_pair(const EpiArgs& e, long row, int col, bool row_ok, float v0, float v1) {
+  constexpr bool kBias = (KIND == EK_BIAS_SOFTPLUS || KIND == EK_BIAS_RELU || KIND == EK_BIAS_GENERIC);
+  const int nmain = kBias ? e.ncol_out : min(e.ncol_out, e.ncol_main);
+  float r0, r1;
+  if constexpr (kBias) {
+    float y0 = v0 + ((e.bias && col < e.n_bias) ? __ldg(e.bias + col) : 0.0f);
+    float y1 = v1 + ((e.bias && col + 1 < e.n_bias) ? __ldg(e.bias + col + 1) : 0.0f);
+    if constexpr (KIND == EK_BIAS_SOFTPLUS) { y0 = softplus100_fast(y0); y1 = softplus100_fast(y1); }
+    else if constexpr (KIND == EK_BIAS_RELU) { y0 = fmaxf(y0, 0.0f); y1 = fmaxf(y1, 0.0f); }
+    else { y0 = apply_act(y0, e.act, e.act_param); y1 = apply_act(y1, e.act, e.act_param); }
+    r0 = e.oscale * y0;
+    r1 = e.oscale * y1;
+  } else {
+    float s0 = 1.0f, s1 = 1.0f;
+    if constexpr (KIND != EK_DACT_NONE) {
+      const float2 h = ld2(e.H, e.ldh, row, col, nmain, row_ok);
+      if constexpr (KIND == EK_DACT_RELU) { s0 = h.x > 0.0f ? 1.0f : 0.0f; s1 = h.y > 0.0f ? 1.0f : 0.0f; }
+      else { s0 = dsoftplus100_fast(h.x, e.hscale); s1 = dsoftplus100_fast(h.y, e.hscale); }
+    }
+    r0 = e.oscale * s0 * v0;
+    r1 = e.oscale * s1 * v1;
+    if constexpr (KIND == EK_TANGENT) {
+      const float2 v = ld2(e.V, e.ldv, row, col, nmain, row_ok);
+      st2(e.out2, e.ldo2, row, col, nmain, row_ok, 100.0f * (1.0f - s0) * v.x * v0, 100.0f * (1.0f - s1) * v.y * v1);
+    }
+    if (e.addend) {
+      const float2 a = ld2(e.addend, e.ldadd, row, col, nmain, row_ok);
+      r0 += a.x;
+      r1 += a.y;
+    }
+    // skip-branch columns [ncol_main, ncol_out) carry oscale * acc and go to the tail buffer
+    if (e.tail && row_ok) {
+      if (col >= e.ncol_main && col < e.ncol_out) e.tail[row * e.ldt + (col - e.ncol_main)] = e.oscale * v0;
+      if (col + 1 >= e.ncol_main && col + 1 < e.ncol_out) e.tail[row * e.ldt + (col + 1 - e.ncol_main)] = e.oscale * v1;
+    }
+  }
+  st2(e.out, e.ldo, row, col, nmain, row_ok, r0, r1);
+  return make_float2(col < nmain ? r0 : 0.0f, col + 1 < nmain ? r1 : 0.0f);
+}
+
+}  // namespace nero

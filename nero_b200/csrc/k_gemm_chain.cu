@@ -1,0 +1,282 @@
+// Fused MLP-CHAIN kernel on wgmma: a 128-row tile of samples flows through a whole sequence of linear layers without its
+// activations ever leaving the SM between layers.
+//
+//   Shared memory: the A operand of the current layer as split-bf16 (hi and lo planes, K-major SWIZZLE_128B, up to 256 K
+//   columns = 128 KB) and a ring of kWStages weight stages.  Two consumer warpgroups own 64 rows each: per layer they issue,
+//   per 16-wide k-step, A_lo*W_hi + A_hi*W_lo + A_hi*W_hi into fp32 accumulators in registers (wgmma.m64n128k16 over the
+//   layer's N range in one or two halves of 128 columns: a narrower layer computes columns it never reads back, one MMA
+//   shape keeps the kernel within the register file), then apply bias/activation or the derivative products of the
+//   gradient sweeps to those registers, store what the layer saves to HBM, and write the NEXT layer's A operand over the
+//   current one (each warp only touches its own rows, whose MMAs it has waited for).
+//   The weights stream from L2 as pre-swizzled images: one stage = the hi and lo planes of one 64-wide K chunk for one half
+//   of the N range (up to 32 KB, cp.async.bulk), kWStages ahead of the MMAs across layers and tiles.  Thread 0 refills a
+//   stage as soon as both warpgroups have released it.  (No separate producer warp: at 256 threads a consumer thread may
+//   hold 255 registers, which the two 64-wide fp32 accumulator halves need; 288 or 384 threads cap it at 168 and spill.)
+//
+// This realises SURVEY.md K2/K3/K4/K10/K13 "activations stay on-chip across layers".
+//
+// Skip connection of the SDF network (field.py:139-140): a layer with `csrc` set takes columns >= ncol_out of the
+// next A operand from that buffer, where ray_fill / pe_tangent pre-stored PE/sqrt2 resp. its tangent.
+#include "gemm_common.cuh"
+
+namespace nero {
+
+constexpr int kMaxChainLayers = 10;
+
+// ---------------------------------------------------------------------------------------------- C ABI (host) structs
+struct ChainLayer {
+  const uint8_t* wimg; const float* bias;
+  float* save; const float* H; const float* addend; const float* V; float* out2; float* tail;
+  int n_pad, k_chunks, n_bias, ncol_out, ncol_main, kind, act;
+  int ld_save, ldh, ldadd, ldv, ldo2, ldt;
+  float oscale, hscale, act_param;
+  int write_a, a_blocks;      // write_a: the output becomes the next A operand; a_blocks: 16-col blocks of it to define
+  const float* csrc; int ld_csrc;   // skip-concat source: columns >= ncol_out of the next A operand come from csrc[row, col]
+  int pad_;
+};
+struct ChainParams {
+  const float* A0; int lda0; int k_valid0;
+  int n_layers; const int* m_ptr; int m_cap;
+  ChainLayer L[kMaxChainLayers];
+};
+
+// ---------------------------------------------------------------------------------------------- configuration
+constexpr int CH_BM = 128;
+constexpr int kChThreads = 2 * 128;                 // two warpgroups of 64 rows
+constexpr int kWStages = 3;
+constexpr int HN = 128;                             // accumulator columns per N half
+constexpr uint32_t kHalfBytes = HN * 128;           // one plane of 128 weight rows x 64 K
+constexpr uint32_t kWStageBytes = 2 * kHalfBytes;   // hi + lo planes
+constexpr uint32_t kAPlane = CH_BM * 128;           // one bf16 plane of one 64-wide K chunk of the A operand (16 KB)
+constexpr uint32_t kABytes = 4 * 2 * kAPlane;       // K <= 256: four chunks x (hi, lo)
+constexpr uint32_t kChSmemBytes = kABytes + kWStages * kWStageBytes + 1024 /*align*/ + 64 /*barriers*/;
+static_assert(kChSmemBytes <= 232448, "shared memory budget");
+
+// columns (col, col + 1) of A row r (tile-local) as split-bf16
+__device__ __forceinline__ void put_a2(uint8_t* s_a, int r, int col, float y0, float y1) {
+  uint32_t hi, lo;
+  split2(y0, y1, hi, lo);
+  uint8_t* q = s_a + (col >> 6) * (2 * kAPlane) + sw128_offset(r, col & 63);
+  *reinterpret_cast<uint32_t*>(q) = hi;
+  *reinterpret_cast<uint32_t*>(q + kAPlane) = lo;
+}
+__device__ __forceinline__ float csrc_at(const ChainLayer& L, long row, int col, bool row_ok) {
+  return (L.csrc && row_ok) ? __ldg(L.csrc + row * L.ld_csrc + col) : 0.0f;
+}
+
+// position of the next weight stage to load in the (tile, layer, N half, K chunk) sequence the MMAs walk
+struct WCursor {
+  int tile, li, hf, kc, g;
+};
+struct ConsumerCtx {
+  uint8_t* s_a; uint8_t* s_w; uint64_t* full; uint64_t* empty;
+  int wg, w, l;
+  int g;                      // weight stages consumed so far
+  bool producer;              // thread 0: loads the weight stages
+  WCursor q;
+  int num_tiles;
+};
+
+// load the next weight stage into its ring slot once both warpgroups have released the slot's previous contents
+__device__ __forceinline__ void w_issue(const ChainParams& p, ConsumerCtx& c) {
+  WCursor& q = c.q;
+  if (q.tile >= c.num_tiles) return;
+  const ChainLayer& L = p.L[q.li];
+  const int nh = L.n_pad > HN ? 2 : 1;
+  const uint32_t plane = uint32_t(L.n_pad) * 128u;
+  const int s = q.g % kWStages;
+  mbar_wait(&c.empty[s], ((q.g / kWStages) & 1) ^ 1);
+  // rows [hf*128, +rows) of the chunk's hi plane and of its lo plane; stage rows beyond them only feed unused columns
+  const uint32_t bytes = min(kHalfBytes, plane - q.hf * kHalfBytes);
+  const uint8_t* src = L.wimg + size_t(q.kc) * 2u * plane + size_t(q.hf) * kHalfBytes;
+  mbar_arrive_expect_tx(&c.full[s], 2u * bytes);
+  bulk_copy_g2s(c.s_w + s * kWStageBytes, src, bytes, &c.full[s]);
+  bulk_copy_g2s(c.s_w + s * kWStageBytes + kHalfBytes, src + plane, bytes, &c.full[s]);
+  ++q.g;
+  if (++q.kc == L.k_chunks) {
+    q.kc = 0;
+    if (++q.hf == nh) {
+      q.hf = 0;
+      if (++q.li == p.n_layers) { q.li = 0; q.tile += gridDim.x; }
+    }
+  }
+}
+// this warp is done with weight stage s (its MMAs reading it have completed)
+__device__ __forceinline__ void w_release(const ChainParams& p, ConsumerCtx& c, int s) {
+  if (c.l == 0) mbar_arrive(&c.empty[s]);
+  if (c.producer) w_issue(p, c);
+  __syncwarp();
+}
+
+// the MMAs of one layer followed by its epilogue, for this thread's warpgroup
+template <int KIND>
+__device__ __forceinline__ void chain_layer(const ChainParams& p, const ChainLayer& L, ConsumerCtx& c, int tile, int rows_valid) {
+  constexpr bool kBias = (KIND == EK_BIAS_SOFTPLUS || KIND == EK_BIAS_RELU || KIND == EK_BIAS_GENERIC);
+  const int nh = L.n_pad > HN ? 2 : 1;
+  float acc[2][HN / 2];
+  int prev = -1;
+#pragma unroll
+  for (int hf = 0; hf < 2; ++hf) {
+    if (hf >= nh) break;
+    for (int kc = 0; kc < L.k_chunks; ++kc, ++c.g) {
+      const int s = c.g % kWStages;
+      mbar_wait(&c.full[s], (c.g / kWStages) & 1);
+      const uint32_t a_hi = smem_u32(c.s_a) + kc * (2 * kAPlane) + c.wg * 64 * 128, a_lo = a_hi + kAPlane;
+      const uint32_t b_hi = smem_u32(c.s_w) + s * kWStageBytes, b_lo = b_hi + kHalfBytes;
+      fence_regs<HN / 2>(acc[hf]);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        mma_split3<HN, 0, 0>(acc[hf], make_desc_k_sw128(a_hi + 32 * k), make_desc_k_sw128(a_lo + 32 * k), make_desc_k_sw128(b_hi + 32 * k),
+                             make_desc_k_sw128(b_lo + 32 * k), (kc | k) != 0);
+      wgmma_commit();
+      wgmma_wait<1>();
+      fence_regs<HN / 2>(acc[hf]);
+      if (prev >= 0) w_release(p, c, prev);     // the stage read by the previous group is free
+      prev = s;
+    }
+  }
+  wgmma_wait<0>();
+  fence_regs<HN / 2>(acc[0]);
+  if (nh > 1) fence_regs<HN / 2>(acc[1]);
+  w_release(p, c, prev);
+  // every MMA of the layer that reads this warpgroup's A rows has completed before any of them is overwritten
+  named_bar(1 + c.wg, 128);
+
+  const EpiArgs e{L.bias, L.n_bias, L.save, L.ld_save, L.H, L.ldh, L.hscale, KIND == EK_TANGENT ? nullptr : L.addend, L.ldadd,
+                  L.V, L.ldv, L.out2, L.ldo2, L.tail, L.ldt, L.ncol_out, L.ncol_main, L.oscale, L.act, L.act_param};
+  const int nmain = kBias ? L.ncol_out : min(L.ncol_out, L.ncol_main);
+  const int n_a = L.write_a ? max(L.a_blocks * 16, L.n_pad) : 0;       // next-A columns to define
+#pragma unroll
+  for (int hf = 0; hf < 2; ++hf) {
+    if (hf >= nh) break;
+#pragma unroll
+    for (int jb = 0; jb < HN / 8; ++jb) {
+      const int col = hf * HN + 8 * jb + 2 * (c.l & 3);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int rl = c.wg * 64 + c.w * 16 + (c.l >> 2) + 8 * h;
+        const long row = long(tile) * CH_BM + rl;
+        const bool row_ok = rl < rows_valid;
+        float2 r = make_float2(0.f, 0.f);
+        if (col < L.ncol_out) r = epi_pair<KIND>(e, row, col, row_ok, acc[hf][4 * jb + 2 * h], acc[hf][4 * jb + 2 * h + 1]);
+        if (col < n_a) {
+          if (col >= nmain) r.x = csrc_at(L, row, col, row_ok);
+          if (col + 1 >= nmain) r.y = csrc_at(L, row, col + 1, row_ok);
+          put_a2(c.s_a, rl, col, r.x, r.y);
+        }
+      }
+    }
+  }
+  // next-A columns beyond the accumulator (skip-concat source or zero): each warp fills its own 16 rows
+  const int extra = (n_a - L.n_pad) >> 1;
+  for (int i = c.l; i < 16 * extra; i += 32) {
+    const int rl = c.wg * 64 + c.w * 16 + i / extra, col = L.n_pad + 2 * (i % extra);
+    const long row = long(tile) * CH_BM + rl;
+    const bool row_ok = rl < rows_valid;
+    put_a2(c.s_a, rl, col, csrc_at(L, row, col, row_ok), csrc_at(L, row, col + 1, row_ok));
+  }
+  fence_proxy_async_smem();
+  named_bar(1 + c.wg, 128);
+}
+
+// FAM: 0 = bias/activation epilogues (forward chains), 1 = derivative-product epilogues (gradient sweeps), 2 = tangent
+// sweep.  One instantiation per family keeps the code of each kernel small.
+template <int FAM>
+__global__ void __launch_bounds__(kChThreads, 1) gemm_chain_kernel(const __grid_constant__ ChainParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* s_a = smem;
+  uint8_t* s_w = smem + kABytes;
+  uint64_t* full = reinterpret_cast<uint64_t*>(s_w + kWStages * kWStageBytes);   // [kWStages]  W stage landed
+  uint64_t* empty = full + kWStages;                                             // [kWStages]  W stage consumed (8 warps)
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  int M = p.m_ptr ? *p.m_ptr : p.m_cap;
+  if (M > p.m_cap) M = p.m_cap;
+  const int num_tiles = (M + CH_BM - 1) / CH_BM;
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kWStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  ConsumerCtx c{s_a, s_w, full, empty, warp >> 2, warp & 3, lane, 0, threadIdx.x == 0, WCursor{int(blockIdx.x), 0, 0, 0, 0}, num_tiles};
+  if (c.producer)
+    for (int i = 0; i < kWStages; ++i) w_issue(p, c);
+  const int a0_cols = p.L[0].k_chunks * 64;        // every column the first layer's MMAs read (zeros beyond k_valid0)
+  const bool a0_vec = (reinterpret_cast<uintptr_t>(p.A0) & 15) == 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const int rows_valid = min(CH_BM, M - tile * CH_BM);
+    // ---- first A operand: fp32 rows from HBM -> split-bf16; each warp converts its own 16 rows
+    {
+      const int n4 = a0_cols / 4;
+      for (int i = lane; i < 16 * n4; i += 32) {
+        const int rl = c.wg * 64 + c.w * 16 + i / n4, col = 4 * (i % n4);
+        const long row = long(tile) * CH_BM + rl;
+        float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (rl < rows_valid && col < p.k_valid0) {
+          const float* q = p.A0 + row * p.lda0 + col;
+          if (a0_vec) x = __ldg(reinterpret_cast<const float4*>(q));      // k_valid0 and lda0 are multiples of 4
+          else { x.x = __ldg(q); x.y = __ldg(q + 1); x.z = __ldg(q + 2); x.w = __ldg(q + 3); }
+        }
+        put_a2(s_a, rl, col, x.x, x.y);
+        put_a2(s_a, rl, col + 2, x.z, x.w);
+      }
+      fence_proxy_async_smem();
+      named_bar(1 + c.wg, 128);
+    }
+    for (int li = 0; li < p.n_layers; ++li) {
+      const ChainLayer& L = p.L[li];
+      if constexpr (FAM == 0) {
+        if (L.kind == EK_BIAS_SOFTPLUS) chain_layer<EK_BIAS_SOFTPLUS>(p, L, c, tile, rows_valid);
+        else if (L.kind == EK_BIAS_RELU) chain_layer<EK_BIAS_RELU>(p, L, c, tile, rows_valid);
+        else chain_layer<EK_BIAS_GENERIC>(p, L, c, tile, rows_valid);
+      } else if constexpr (FAM == 1) {
+        if (L.kind == EK_DACT_SOFTPLUS) chain_layer<EK_DACT_SOFTPLUS>(p, L, c, tile, rows_valid);
+        else if (L.kind == EK_DACT_RELU) chain_layer<EK_DACT_RELU>(p, L, c, tile, rows_valid);
+        else chain_layer<EK_DACT_NONE>(p, L, c, tile, rows_valid);
+      } else {
+        chain_layer<EK_TANGENT>(p, L, c, tile, rows_valid);
+      }
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------- host side
+int chain_dispatch(const ChainParams& p, cudaStream_t stream) {
+  if (p.n_layers <= 0 || p.n_layers > kMaxChainLayers || (p.lda0 & 3) || (p.k_valid0 & 3) || p.k_valid0 > 256 || !p.A0) return NERO_ERR_ARG;
+  for (int l = 0; l < p.n_layers; ++l) {
+    const ChainLayer& L = p.L[l];
+    if (L.n_pad % 16 || L.n_pad < 16 || L.n_pad > 256) return NERO_ERR_ARG;
+    if (L.k_chunks < 1 || L.k_chunks > 4 || L.ncol_out > L.n_pad || !L.wimg) return NERO_ERR_ARG;
+    if (L.write_a && (L.a_blocks > 16 || (l + 1 < p.n_layers && L.a_blocks < 4 * p.L[l + 1].k_chunks))) return NERO_ERR_ARG;
+    if (L.kind == EK_TANGENT && (!L.H || !L.V || !L.out2)) return NERO_ERR_ARG;
+    if ((L.kind == EK_DACT_SOFTPLUS || L.kind == EK_DACT_RELU) && !L.H) return NERO_ERR_ARG;
+  }
+  int fam = -1;
+  for (int l = 0; l < p.n_layers; ++l) {
+    const int k = p.L[l].kind;
+    const int f = k <= EK_BIAS_GENERIC ? 0 : (k == EK_TANGENT ? 2 : 1);
+    if (fam >= 0 && f != fam) return NERO_ERR_ARG;   // a chain is homogeneous: forward, gradient sweep or tangent sweep
+    fam = f;
+  }
+  const int tiles_cap = (p.m_cap + CH_BM - 1) / CH_BM;
+  if (tiles_cap <= 0) return NERO_OK;
+  static bool attr_set = false;
+  if (!attr_set) {
+    if (cudaFuncSetAttribute(gemm_chain_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kChSmemBytes) != cudaSuccess ||
+        cudaFuncSetAttribute(gemm_chain_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kChSmemBytes) != cudaSuccess ||
+        cudaFuncSetAttribute(gemm_chain_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kChSmemBytes) != cudaSuccess)
+      return NERO_ERR_CUDA;
+    attr_set = true;
+  }
+  const int grid = tiles_cap < kNumSMs ? tiles_cap : kNumSMs;
+  if (fam == 0) gemm_chain_kernel<0><<<grid, kChThreads, kChSmemBytes, stream>>>(p);
+  else if (fam == 1) gemm_chain_kernel<1><<<grid, kChThreads, kChSmemBytes, stream>>>(p);
+  else gemm_chain_kernel<2><<<grid, kChThreads, kChSmemBytes, stream>>>(p);
+  NERO_LAUNCH_CHECK();
+  return NERO_OK;
+}
+
+}  // namespace nero

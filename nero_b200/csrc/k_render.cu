@@ -320,6 +320,11 @@ __global__ void sdf_alpha_fwd_kernel(const float* __restrict__ Y8, int ldy, int 
   gerr[i] = o.grad_err;
 }
 
+// d inv_s is a sum over all samples: each block writes its warp-ordered partial to dinvs_partials[block] and
+// sdf_alpha_bwd_finish_kernel adds them up in a fixed order, so the result is the same every run (no floating-point atomics)
+constexpr int kDinvsMaxBlocks = 65536;
+__device__ float dinvs_partials[kDinvsMaxBlocks];
+
 __global__ void sdf_alpha_bwd_kernel(const float* __restrict__ Y8, int ldy, int sdf_col, const float* __restrict__ G,
                                      const float* __restrict__ pts, const int* __restrict__ ray_in,
                                      const float* __restrict__ rays_d, const float* variance, const float* car_p,
@@ -343,8 +348,27 @@ __global__ void sdf_alpha_bwd_kernel(const float* __restrict__ Y8, int ldy, int 
     dY8[size_t(i) * lddy + sdf_col] = dsdf;
     *reinterpret_cast<float4*>(DG + size_t(i) * 4) = make_float4(dg[0], dg[1], dg[2], 0.f);
   }
+  __shared__ float s_w[32];
   for (int o = 16; o > 0; o >>= 1) dis += __shfl_xor_sync(0xffffffffu, dis, o);
-  if ((threadIdx.x & 31) == 0 && dis != 0.0f) atomicAdd(d_inv_s, dis);
+  if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = dis;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float t = 0.0f;
+    for (int wi = 0; wi < int(blockDim.x >> 5); ++wi) t += s_w[wi];
+    dinvs_partials[blockIdx.x] = t;
+  }
+}
+__global__ void sdf_alpha_bwd_finish_kernel(int nparts, float* d_inv_s) {
+  __shared__ float s_t[256];
+  float t = 0.0f;
+  for (int i = threadIdx.x; i < nparts; i += blockDim.x) t += dinvs_partials[i];
+  s_t[threadIdx.x] = t;
+  __syncthreads();
+  for (int h = blockDim.x >> 1; h > 0; h >>= 1) {
+    if (int(threadIdx.x) < h) s_t[threadIdx.x] += s_t[threadIdx.x + h];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *d_inv_s += s_t[0];
 }
 
 // ------------------------------------------------------------------ outer NeRF post
@@ -515,7 +539,10 @@ int sdf_alpha_backward(const float* Y8, int ldy, int sdf_col, const float* G, co
                        const float* variance, const float* car, const float* dalpha, const float* dgerr, float* dY8, int lddy, float* DG,
                        float* d_inv_s, const int* m_ptr, int m_cap, cudaStream_t st) {
   if (m_cap <= 0) return NERO_OK;
-  sdf_alpha_bwd_kernel<<<blocks_for(m_cap, 256), 256, 0, st>>>(Y8, ldy, sdf_col, G, pts, ray_in, rays_d, variance, car, dalpha, dgerr, dY8, lddy, DG, d_inv_s, m_ptr, m_cap);
+  const int nb = blocks_for(m_cap, 256);
+  if (nb > kDinvsMaxBlocks) return NERO_ERR_ARG;
+  sdf_alpha_bwd_kernel<<<nb, 256, 0, st>>>(Y8, ldy, sdf_col, G, pts, ray_in, rays_d, variance, car, dalpha, dgerr, dY8, lddy, DG, d_inv_s, m_ptr, m_cap);
+  sdf_alpha_bwd_finish_kernel<<<1, 256, 0, st>>>(nb, d_inv_s);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }

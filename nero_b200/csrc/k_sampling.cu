@@ -236,8 +236,13 @@ __global__ void occ_init_kernel(const float* __restrict__ pts, const float* __re
   for (int c = 0; c < 39; ++c) { x0[c] = pe[c]; hc[217 + c] = pe[c] * kInvSqrt2s; }
 }
 
-// candidate mask of the occlusion loss (renderer.py:530-533) and compaction: block-local ordered scan + one atomic
-// per block for the base offset (the order across blocks is irrelevant: the loss is a mean over the selected set)
+// candidate mask of the occlusion loss (renderer.py:530-533) and compaction in sample order, in two passes: pass 0 stores
+// each block's candidate count, pass 1 recomputes the mask and writes the candidates at the block's offset (the sum of the
+// counts of the blocks before it).  The list is the same every run, so is the random subset drawn from it.
+constexpr int kOccMaxBlocks = 16384;
+__device__ int occ_block_counts[kOccMaxBlocks];
+
+template <int PASS>
 __global__ void occ_select_kernel(const float* __restrict__ pts, const float* __restrict__ Y8, int ldy, int sdf_col,
                                   const float* __restrict__ G, const int* __restrict__ ray_in, const float* __restrict__ rays_d,
                                   float sdf_thresh, const int* m_ptr, int m_cap, int* sel, int* count) {
@@ -267,27 +272,44 @@ __global__ void occ_select_kernel(const float* __restrict__ pts, const float* __
     int incl = v;
     for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
     s_warp[lane] = incl - v;
-    if (lane == 31) s_base = incl > 0 ? atomicAdd(count, incl) : 0;
+    if (PASS == 0 && lane == 31) occ_block_counts[blockIdx.x] = incl;
+    if (PASS == 1) {
+      int base = 0;
+      for (int b = lane; b < int(blockIdx.x); b += 32) base += occ_block_counts[b];
+      for (int o = 16; o > 0; o >>= 1) base += __shfl_xor_sync(0xffffffffu, base, o);
+      if (lane == 31) {
+        s_base = base;
+        if (blockIdx.x == gridDim.x - 1) *count = base + incl;
+      }
+    }
   }
+  if (PASS == 0) return;
   __syncthreads();
   if (flag) sel[s_base + s_warp[warp] + wrank] = i;
 }
 
-// L1 occlusion loss pieces: loss_sum += |occ_prob[sel] - gt| ; docc[sel] = sign(..) (scaled by 1/P on the host side)
+// L1 occlusion loss pieces: loss_sum += |occ_prob[sel] - gt| ; docc[sel] = sign(..) (scaled by 1/P on the host side).
+// One block, summed in a fixed order (the subset holds at most a few thousand points).
+constexpr int kOccLossThreads = 1024;
 __global__ void occ_loss_kernel(const float* __restrict__ occ_prob, const float* __restrict__ gt, const int* __restrict__ sel,
                                 const int* p_ptr, int p_cap, float* loss_sum, float* docc_sign) {
+  __shared__ float s_l[kOccLossThreads];
   int P = p_ptr ? *p_ptr : p_cap;
   if (P > p_cap) P = p_cap;
-  const int pi = blockIdx.x * blockDim.x + threadIdx.x;
   float l = 0.f;
-  if (pi < P) {
+  for (int pi = threadIdx.x; pi < P; pi += blockDim.x) {
     const int i = sel[pi];
     const float df = occ_prob[i] - gt[pi];
-    l = fabsf(df);
+    l += fabsf(df);
     docc_sign[i] = df > 0.f ? 1.0f : (df < 0.f ? -1.0f : 0.0f);
   }
-  for (int o = 16; o > 0; o >>= 1) l += __shfl_xor_sync(0xffffffffu, l, o);
-  if ((threadIdx.x & 31) == 0 && l != 0.f) atomicAdd(loss_sum, l);
+  s_l[threadIdx.x] = l;
+  __syncthreads();
+  for (int h = blockDim.x >> 1; h > 0; h >>= 1) {
+    if (int(threadIdx.x) < h) s_l[threadIdx.x] += s_l[threadIdx.x + h];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *loss_sum += s_l[0];
 }
 
 static inline int blocks_for(long n, int per) { return int((n + per - 1) / per); }
@@ -324,15 +346,17 @@ int occ_init(const float* pts, const float* refl, const int* sel, const int* p_p
 int occ_select(const float* pts, const float* Y8, int ldy, int sdf_col, const float* G, const int* ray_in, const float* rays_d,
                float sdf_thresh, const int* m_ptr, int m_cap, int* sel, int* count, cudaStream_t st) {
   if (m_cap <= 0) return NERO_OK;
-  NERO_CUDA_TRY(cudaMemsetAsync(count, 0, sizeof(int), st));
-  occ_select_kernel<<<blocks_for(m_cap, 1024), 1024, 0, st>>>(pts, Y8, ldy, sdf_col, G, ray_in, rays_d, sdf_thresh, m_ptr, m_cap, sel, count);
+  const int nb = blocks_for(m_cap, 1024);
+  if (nb > kOccMaxBlocks) return NERO_ERR_ARG;
+  occ_select_kernel<0><<<nb, 1024, 0, st>>>(pts, Y8, ldy, sdf_col, G, ray_in, rays_d, sdf_thresh, m_ptr, m_cap, sel, count);
+  occ_select_kernel<1><<<nb, 1024, 0, st>>>(pts, Y8, ldy, sdf_col, G, ray_in, rays_d, sdf_thresh, m_ptr, m_cap, sel, count);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
 int occ_loss(const float* occ_prob, const float* gt, const int* sel, const int* p_ptr, int p_cap, float* loss_sum, float* docc_sign,
              cudaStream_t st) {
   if (p_cap <= 0) return NERO_OK;
-  occ_loss_kernel<<<blocks_for(p_cap, 256), 256, 0, st>>>(occ_prob, gt, sel, p_ptr, p_cap, loss_sum, docc_sign);
+  occ_loss_kernel<<<1, kOccLossThreads, 0, st>>>(occ_prob, gt, sel, p_ptr, p_cap, loss_sum, docc_sign);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }

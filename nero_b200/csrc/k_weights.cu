@@ -9,7 +9,7 @@
 // kmap[k] of the (padded / re-ordered) activation layout the kernels actually use; `in_scale` folds constant
 // input scalings.  Images must be zero-initialised once (padding stays zero).
 //
-// nero_wgrad_finish: reduces the split-K partials of k_umma_wgrad.cu, maps layout columns back through kmap and
+// nero_wgrad_finish: reduces the split-K partials of k_gemm_wgrad.cu, maps layout columns back through kmap and
 // accumulates into .grad of (weight_g, weight_v, bias) via the weight-norm chain rule, or (weight, bias).
 #include "common.cuh"
 
@@ -178,9 +178,8 @@ __global__ void wgrad_finish_batch_kernel(const FinishJob* __restrict__ jobs) {
 int wgrad_finish_batch(const void* jobs_dev, int n_jobs, int max_rows, int max_k, cudaStream_t stream) {
   if (n_jobs <= 0 || max_rows <= 0) return NERO_OK;
   if (!jobs_dev || max_k <= 0 || max_k > 1024) return NERO_ERR_ARG;
-  // the batched jobs come from the accumulating weight-gradient GEMM (one accumulator, P = 1): a row is ~1.5 KB of work, so
-  // small blocks (many resident per SM) instead of the (256, 4) layout of the split-K reduction
-  wgrad_finish_batch_kernel<<<dim3(max_rows, n_jobs), dim3(128, 1), max_k * sizeof(float), stream>>>(static_cast<const FinishJob*>(jobs_dev));
+  // (256, 4) blocks: four groups of partial slices are summed in parallel (the per-row reads are latency bound)
+  wgrad_finish_batch_kernel<<<dim3(max_rows, n_jobs), dim3(256, 4), 4 * max_k * sizeof(float), stream>>>(static_cast<const FinishJob*>(jobs_dev));
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
@@ -200,8 +199,13 @@ int wgrad_finish(const float* partial, int P, int rows_partial, int ld_partial, 
 
 // column sums: out[j] (+)= sum_m w[m] * X[m, j]   (w may be null = ones).  Used for the sdf row of lin8:
 // dW8[0,:] = sum_m dsdf[m] * h8[m,:] + sum_m ubar8[m,:]   and for its bias.
+// Block row y writes its partial sums to colsum_partials[y]; a second kernel adds them up in a fixed order, so the result
+// is the same every run (no floating-point atomics).
+constexpr int kColsumMaxCols = 1024;
+__device__ float colsum_partials[kNumSMs * kColsumMaxCols];
+
 __global__ void colsum_kernel(const float* __restrict__ X, int ldx, int ncol, const float* __restrict__ w, int ldw,
-                              const int* __restrict__ m_ptr, int m_cap, float* out) {
+                              const int* __restrict__ m_ptr, int m_cap) {
   int M = m_ptr ? *m_ptr : m_cap;
   if (M > m_cap) M = m_cap;
   // 256 threads = 8 row lanes x 32 column lanes of 4 adjacent columns each (one float4 per row and thread)
@@ -243,16 +247,25 @@ __global__ void colsum_kernel(const float* __restrict__ X, int ldx, int ncol, co
       if (col + c >= ncol) break;
       float t = 0.0f;
       for (int i = 0; i < 8; ++i) t += sh[i][lane][c];
-      atomicAdd(out + col + c, t);
+      colsum_partials[blockIdx.y * kColsumMaxCols + col + c] = t;
     }
   }
+}
+__global__ void colsum_finish_kernel(int ncol, int nparts, float* out) {
+  const int col = blockIdx.x * blockDim.x + threadIdx.x;
+  if (col >= ncol) return;
+  float t = 0.0f;
+  for (int y = 0; y < nparts; ++y) t += colsum_partials[y * kColsumMaxCols + col];
+  out[col] += t;
 }
 
 int colsum(const float* X, int ldx, int ncol, const float* w, int ldw, const int* m_ptr, int m_cap, float* out,
            cudaStream_t stream) {
   if (m_cap <= 0 || ncol <= 0) return NERO_OK;
-  dim3 grid((ncol + 127) / 128, 148);
-  colsum_kernel<<<grid, 256, 0, stream>>>(X, ldx, ncol, w, ldw, m_ptr, m_cap, out);
+  if (ncol > kColsumMaxCols) return NERO_ERR_ARG;
+  dim3 grid((ncol + 127) / 128, kNumSMs);
+  colsum_kernel<<<grid, 256, 0, stream>>>(X, ldx, ncol, w, ldw, m_ptr, m_cap);
+  colsum_finish_kernel<<<(ncol + 127) / 128, 128, 0, stream>>>(ncol, kNumSMs, out);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }

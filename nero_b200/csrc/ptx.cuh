@@ -1,24 +1,16 @@
-// Thin inline-PTX wrappers for the sm_100a features the kernels use: mbarrier, bulk async copy (UBLKCP),
-// tcgen05 (TMEM alloc, MMA, commit, ld) and the UMMA shared-memory / instruction descriptors.
+// Thin inline-PTX wrappers for the sm_90a features the kernels use: mbarrier, bulk async copy (UBLKCP), the warpgroup
+// MMA (wgmma) fences and the shared-memory matrix descriptors.
 // Every spin-wait is BOUNDED: a wait that does not complete traps (kernel error) instead of hanging the GPU.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
 
+#include "wgmma.cuh"
+
 namespace nero {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
-
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
 }
 
 // ------------------------------------------------------------------ mbarrier
@@ -46,33 +38,22 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// non-blocking probe (try_wait may suspend the thread for a system-dependent time before it reports failure: a
-// thread that polls SEVERAL barriers must use test_wait)
-__device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 P, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-// Bounded wait: ~2^24 polls (a few seconds) then trap -> the launch fails loudly instead of hanging the box.
+// Bounded wait: ~2^24 polls (a few seconds) then trap -> the launch fails loudly instead of hanging the GPU.  (No printf
+// here: a function call inside the wgmma pipeline makes ptxas serialise every wgmma of the kernel.)
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (++spins > (1u << 24)) {
-      printf("nero: mbarrier wait timeout (block %d thread %d)\n", blockIdx.x, threadIdx.x);
-      __trap();
-    }
+    if (++spins > (1u << 24)) __trap();
   }
 }
 
-// make generic-proxy smem writes visible to the async proxy (tcgen05.mma / bulk copies read smem through it)
+// make generic-proxy smem writes visible to the async proxy (wgmma / bulk copies read smem through it)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+}
+// named barrier over `count` threads (ids 1..15; 0 is __syncthreads)
+__device__ __forceinline__ void named_bar(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
 // ------------------------------------------------------------------ bulk async copy global -> shared (UBLKCP)
@@ -83,86 +64,39 @@ __device__ __forceinline__ void bulk_copy_g2s(void* smem_dst, const void* gmem_s
       : "memory");
 }
 
-// ------------------------------------------------------------------ tcgen05 / TMEM
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {  // one full warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "n"(kCols));
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {  // the same warp that allocated
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols));
-}
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16 x bf16 -> fp32, issued by ONE thread
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// commit all prior MMAs of this thread; arrives on the mbarrier when they complete
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+// ------------------------------------------------------------------ wgmma
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+template <int N>
+__device__ __forceinline__ void fence_regs(float* r) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
 }
 
-// 32 lanes x 32 columns of fp32: thread i of the warp gets TMEM lane (base_lane + i), columns [col, col+32)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ------------------------------------------------------------------ descriptors
-// K-major operand tile, 128-byte swizzle: rows are 128 B (64 bf16) apart, 8-row groups 1024 B apart.
-// (cute::UMMA::SmemDescriptor: start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), version=1 [46,48), layout [61,64))
+// ------------------------------------------------------------------ descriptors (sm_90 GMMA layout)
+// start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), layout [62,64): 1 = SWIZZLE_128B
+// K-major operand tile, 128-byte swizzle: rows are 128 B (64 bf16) apart, 8-row groups 1024 B apart (LBO unused).
 __device__ __forceinline__ uint64_t make_desc_k_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;             // LBO (ignored for swizzled K-major)
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;     // SBO: 8 rows * 128 B
-  d |= static_cast<uint64_t>(1) << 46;             // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;             // SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 16;
+  d |= static_cast<uint64_t>(1024 >> 4) << 32;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-// MN-major operand tile, 128-byte swizzle (cute::UMMA canonical layout ((8,8,m),(8,k)):((1,8,LBO),(64,SBO)) in bf16
-// elements): an atom is 8 K-rows x 64 MN-elements (8 x 128 B, 16-byte chunks XOR-swizzled with the row index); atoms
-// repeat along K every `sbo` bytes and along MN every `lbo` bytes.
+// MN-major operand tile, 128-byte swizzle (canonical layout ((8,8,m),(8,k)):((1,8,LBO),(64,SBO)) in bf16 elements): an
+// atom is 8 K-rows x 64 MN-elements (8 x 128 B, 16-byte chunks XOR-swizzled with the row index); atoms repeat along MN
+// every `lbo` bytes and along K every `sbo` bytes.
 __device__ __forceinline__ uint64_t make_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>(lbo >> 4) << 16;
   d |= static_cast<uint64_t>(sbo >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;             // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;             // SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
-}
-// kind::f16 instruction descriptor: BF16 x BF16 -> F32, both operands K-major, M x N tile
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t M, uint32_t N) {
-  return (1u << 4)                 // c_format  = F32
-         | (1u << 7)               // a_format  = BF16
-         | (1u << 10)              // b_format  = BF16
-         | ((N >> 3) << 17)        // n_dim
-         | ((M >> 4) << 24);       // m_dim
-}
-// same with both operands MN-major (a_major bit 15, b_major bit 16)
-__host__ __device__ constexpr uint32_t make_idesc_bf16_mn(uint32_t M, uint32_t N) {
-  return make_idesc_bf16(M, N) | (1u << 15) | (1u << 16);
 }
 
 }  // namespace nero

@@ -1,6 +1,6 @@
-"""Host-side orchestration of the stage-I hot path on one B200: sample_ray + render_core forward / backward.
+"""Host-side orchestration of the stage-I hot path on one H100: sample_ray + render_core forward / backward.
 
-Python only sequences kernels: every arithmetic step is a hand-written sm_100a kernel reached through the C ABI
+Python only sequences kernels: every arithmetic step is a hand-written sm_90a kernel reached through the C ABI
 (ops.K / ops.linear / ops.wgrad).  Data-dependent sizes (number of inner / outer samples) stay on the device:
 workspaces are sized for the worst case and kernels read the live counts from device memory.
 
@@ -22,7 +22,7 @@ from . import ops
 from .ops import Mat, K, linear, wgrad, chain, chain_layer as CL, ACT_NONE, ACT_SOFTPLUS100, ACT_RELU, ACT_SIGMOID, ACT_EXPCLAMP, EPI_MUL_DACT, EPI_TANGENT
 from .ops import EK_BIAS_SOFTPLUS, EK_BIAS_RELU, EK_BIAS_GENERIC, EK_DACT_SOFTPLUS, EK_DACT_RELU, EK_DACT_NONE, EK_TANGENT
 
-USE_CHAIN = True    # fused MLP-chain kernel (k_umma_chain.cu); False = one nero_linear launch per layer
+USE_CHAIN = True    # fused MLP-chain kernel (k_gemm_chain.cu); False = one nero_linear launch per layer
 
 INV_SQRT2 = 0.7071067811865476
 SQRT2 = 1.4142135623730951

@@ -1,4 +1,4 @@
-"""Stage II (material estimation) on the B200: `NeROMaterialRenderer` with the reference's API.
+"""Stage II (material estimation) on the H100: `NeROMaterialRenderer` with the reference's API.
 
 Reference being replaced (paths relative to /root/reference):
   NeROMaterialRenderer.__init__/trace/shade/train_step   network/renderer.py:666-848

@@ -1,7 +1,7 @@
 """ctypes bindings of libnero_b200.so + thin tensor-level wrappers.
 
 The product path has NO fallback and no alternate backend: importing this module without the built library raises, and
-every wrapper launches a hand-written sm_100a kernel through the C ABI declared in include/nero_b200.h.  (The CPU walk of
+every wrapper launches a hand-written sm_90a kernel through the C ABI declared in include/nero_b200.h.  (The CPU walk of
 the host logic used by the test-suite lives in tests/dry_run_harness.py and works by substituting `lib` from outside.)
 """
 import ctypes
@@ -49,7 +49,7 @@ def npad_for(n):
     for c in _NPADS:
         if n <= c:
             return c
-    raise ValueError(f'width {n} > 256 not supported by one UMMA tile')
+    raise ValueError(f'width {n} > 256 not supported by one MMA tile')
 
 
 def ceil_div(a, b):
@@ -203,18 +203,20 @@ def _finish_job_dtype():
 
 
 class WgradWorkspace:
-    """Accumulators of the weight-gradient GEMMs.  nero_wgrad splits the sample rows over `P` CTAs per output tile; each CTA
-    ADDS its tile into one [rows x ld] fp32 accumulator with L2 reductions (no split-K partial round trip through HBM).
+    """Accumulators of the weight-gradient GEMMs.  nero_wgrad splits the sample rows over `P` CTAs per output tile; CTA p adds
+    its tile into slice p of a [P, rows, ld] fp32 accumulator, and the finish kernel sums the slices in a fixed order, so the
+    gradients are the same every run (no floating-point atomics).
     With `defer` set (the engines do), every nero_wgrad launch gets its own accumulator slot and its weight-norm chain rule is
     queued; `flush()` runs all queued jobs in ONE nero_wgrad_finish_batch launch and re-zeroes the used slots (one memset).
     Jobs that would accumulate into the same gradient rows are never queued together (the queue is flushed first), so the
     batched kernel has no write conflicts."""
 
-    def __init__(self, device, P=74, rows=256, ld=384, max_slots=48):
+    def __init__(self, device, P=66, rows=256, ld=384, max_slots=48):
         self.P, self.rows, self.ld = P, rows, ld
         self.device, self.max_slots = device, max_slots
-        # one pool: slot i = acc[i] [rows, ld] followed by its bias sums [rows]; zero = ready to accumulate into
-        self.pool = torch.zeros(max_slots, rows * ld + rows, dtype=torch.float32, device=device)
+        # slot i = acc[i] [P, rows, ld] followed by its bias sums [P, rows]; zero = ready to accumulate into.  Slots are made
+        # on first use and kept, so their addresses stay valid for graph replay
+        self.slots = []
         self.jobs, self.dest, self.keep = [], set(), []
         self.defer = False
         self._tabs = {}      # device copies of the finish-job tables, keyed by their content: a training step queues the same
@@ -222,8 +224,11 @@ class WgradWorkspace:
 
     def _slot(self):
         i = len(self.jobs)
-        row = self.pool[i]
-        return row[:self.rows * self.ld].view(1, self.rows, self.ld), row[self.rows * self.ld:].view(1, self.rows)
+        while len(self.slots) <= i:
+            self.slots.append(torch.zeros(self.P * (self.rows * self.ld + self.rows), dtype=torch.float32, device=self.device))
+        row = self.slots[i]
+        n = self.P * self.rows * self.ld
+        return row[:n].view(self.P, self.rows, self.ld), row[n:].view(self.P, self.rows)
 
     @property
     def partial(self):
@@ -259,7 +264,7 @@ class WgradWorkspace:
         rc = lib.nero_wgrad_finish_batch(_ptr(tab), len(self.jobs), max_rows, max_k, _stream())
         _check(rc, 'nero_wgrad_finish_batch')
         launch_count += 1
-        self.pool[:len(self.jobs)].zero_()          # the used accumulators are ready for the next pass
+        torch._foreach_zero_(self.slots[:len(self.jobs)])     # the used accumulators are ready for the next pass
         self.jobs, self.dest, self.keep = [], set(), []
 
 
@@ -276,8 +281,7 @@ def wgrad(ws: WgradWorkspace, dY: Mat, n_valid, X: Mat, k_valid, layer: Prepared
     if ws.defer and grad_w is not None and (grad_w.data_ptr(), layer.row0) in ws.dest:
         ws.flush()                      # a queued job already accumulates into these rows
     partial_t, bias_t = ws.partial, ws.bias_partial
-    # row slices per 128-row output tile: all 148 SMs busy also when the layer has a single tile (narrow heads)
-    P = ws.P * 2 // ceil_div(n_rows_pad, 128) if n_rows_pad <= 128 else ws.P
+    P = ws.P          # row slices per 128-row output tile, one accumulator slice each
     if not ws.defer:          # stand-alone use: the accumulator slot is zeroed per call
         partial_t.zero_()
         bias_t.zero_()
@@ -292,10 +296,10 @@ def wgrad(ws: WgradWorkspace, dY: Mat, n_valid, X: Mat, k_valid, layer: Prepared
     if ws.defer:
         ptr = lambda t: 0 if t is None else t.data_ptr()
         job = (ptr(partial_t), ptr(bias_t) if with_bias else 0, ptr(layer.kmap), ptr(w_), ptr(g), ptr(grad_w), ptr(grad_g),
-               ptr(grad_b) if with_bias else 0, 0, 1, ws.rows, ws.ld, layer.K, layer.row0, layer.nrows, 1.0, 0.0)
+               ptr(grad_b) if with_bias else 0, 0, P, ws.rows, ws.ld, layer.K, layer.row0, layer.nrows, 1.0, 0.0)
         ws.enqueue(job, (grad_w.data_ptr(), layer.row0), (w_, g))
         return
-    rc = lib.nero_wgrad_finish(_ptr(partial_t), 1, ws.rows, ws.ld, _ptr(bias_t) if with_bias else None,
+    rc = lib.nero_wgrad_finish(_ptr(partial_t), P, ws.rows, ws.ld, _ptr(bias_t) if with_bias else None,
                                layer.K, layer.row0, layer.nrows, _ptr(layer.kmap), ctypes.c_float(1.0),
                                _ptr(w_), _ptr(g), _ptr(grad_w), _ptr(grad_g),
                                _ptr(grad_b) if with_bias else None, None, ctypes.c_float(0.0), _stream())
@@ -411,7 +415,7 @@ PROFILE = None   # bench.py: list collecting (tag, event0, event1, flops_per_row
 
 
 def chain(A0: Mat, k_valid0, layers, m_ptr=None, m_cap=None, tag=''):
-    """Run consecutive layers on each 128-row tile with the A operand kept in TMEM (k_umma_chain.cu)."""
+    """Run consecutive layers on each 128-row tile with the A operand kept in shared memory (k_gemm_chain.cu)."""
     global launch_count
     assert 1 <= len(layers) <= 10
     if m_cap is None:

@@ -1,5 +1,5 @@
 """Drop-in replacements for the reference's renderers (network/renderer.py): same registry name, constructor,
-cfg keys, forward(data) contract, output dictionaries and state_dict layout -- backed by the sm_100a kernels of
+cfg keys, forward(data) contract, output dictionaries and state_dict layout -- backed by the sm_90a kernels of
 libnero_b200 instead of PyTorch ops.
 
     from nero_b200.renderer import name2renderer      # {'shape': NeROShapeRenderer, ...}

@@ -33,14 +33,18 @@ def test_no_cpu_fallback():
         net.sample_ray(o, o, o[:, :1], o[:, :1], 0)
 
 
-def test_sass_uses_blackwell_tensor_path():
-    """cuobjdump: the library must contain UTCHMMA (tcgen05.mma), LDTM (tcgen05.ld) and UBLKCP (bulk copy)."""
+def test_sass_uses_hopper_tensor_path():
+    """cuobjdump: the library is sm_90a code and contains HGMMA (wgmma.mma_async) and UBLKCP (bulk copy)."""
     import subprocess
     import __graft_entry__ as g
-    out = subprocess.run(['cuobjdump', '-sass', g.build()], capture_output=True, text=True).stdout
-    for mnemonic in ('UTCHMMA', 'LDTM', 'UBLKCP'):
+    lib = g.build()
+    out = subprocess.run(['cuobjdump', '-sass', lib], capture_output=True, text=True).stdout
+    for mnemonic in ('HGMMA', 'UBLKCP'):
         assert mnemonic in out, mnemonic
-    assert 'HMMA.' not in out.replace('UTCHMMA', ''), 'legacy mma.sync path must not be used'
+    assert 'HMMA.' not in out.replace('HGMMA', ''), 'legacy mma.sync path must not be used'
+    elfs = subprocess.run(['cuobjdump', '-lelf', lib], capture_output=True, text=True).stdout.split()
+    cubins = [e for e in elfs if e.endswith('.cubin')]
+    assert cubins and all(e.endswith('.sm_90a.cubin') for e in cubins), cubins
 
 
 def test_binding_struct_layouts_match_the_library():

@@ -66,7 +66,7 @@ def _shape_case(cfg, R, steps):
             out = net.render_core(r['rays_o'], r['rays_d'], z, r['human_poses'], car, step, perm=perm.to(DEV))
             ref = O.render_core(sd, c, lut, rays['rays_o'], rays['rays_d'], zc, rays['human_poses'], car, step, perm=perm)
         n_in = net.engine.state['N_in']
-        assert (n_in + 127) // 128 > 4 * 148, 'every persistent CTA must loop over several row tiles in this test'
+        assert (n_in + 127) // 128 > 4 * 132, 'every persistent CTA must loop over several row tiles in this test'
         assert ref['gradient_error'].shape[0] == n_in, 'inner / outer classification differs from the oracle'
         _close(out['ray_rgb'], ref['ray_rgb'], 1e-4, 2e-5, f'ray_rgb (R={R}, step {step})')
         v, e = _viol(out['gradient_error'], ref['gradient_error'], 2e-3, 2e-5)

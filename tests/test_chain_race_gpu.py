@@ -1,10 +1,10 @@
-"""Run-to-run determinism of the fused MLP-chain kernel under cold weights (regression test of a shared-memory race).
+"""Run-to-run determinism of the fused MLP-chain kernel under cold weights (regression test of shared-memory races).
 
-The chain kernel double-buffers each layer's bias in shared memory.  Indexed by (layer & 1), a chain with an ODD number of
-layers used the same buffer for the last layer of one 128-row tile and the first layer of the next one: an epilogue warp
-that was one A0 conversion ahead overwrote the bias the slower warps were still adding.  It only showed with several tiles
-per CTA and weight images cold in L2 (as in a training step, where the backward pass evicts them): rare, grossly wrong SDF
-values in the 9-layer sampling chain.  Here: the same launch 200 times with an L2 flush in between, bit-identical outputs."""
+The chain kernel streams weight stages through a ring shared by two warpgroups and rewrites each tile's A operand in place
+between layers; a stage refilled, or an A row overwritten, before every MMA reading it has completed gives rare, grossly wrong
+SDF values of the 9-layer sampling chain.  Such races only show with several tiles per CTA and weight images cold in L2 (as
+in a training step, where the backward pass evicts them).  Here: the same launch 200 times with an L2 flush in between,
+bit-identical outputs."""
 import pytest
 import torch
 
@@ -21,7 +21,7 @@ def test_sampling_chain_is_bit_reproducible_with_cold_weights():
     net = net.cuda()
     e = net.engine
     e.prepare_weights()
-    rows = 65536                                    # 512 tiles over 148 CTAs: 3-4 tiles per CTA
+    rows = 65536                                    # 512 tiles over 132 CTAs: 3-4 tiles per CTA
     e._alloc(1024, 160)
     w = e.w
     g = torch.Generator(device=dev).manual_seed(5)
@@ -30,7 +30,7 @@ def test_sampling_chain_is_bit_reproducible_with_cold_weights():
     w['SX0'][:rows].copy_(X)
     w['SC'][:rows, 217:256].copy_(X[:, :39] * 0.70710678)
     out = torch.zeros(rows, 1, device=dev)
-    flush = torch.empty(96 * 1024 * 1024, device=dev)       # 384 MB > the 126 MB L2
+    flush = torch.empty(96 * 1024 * 1024, device=dev)       # 384 MB > the 50 MB L2
 
     def run():
         flush.fill_(1.0)

@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 GEMM kernels (nero_linear / nero_wgrad) against fp64 torch on the same inputs.
+"""GPU parity of the wgmma GEMM kernels (nero_linear / nero_wgrad) against fp64 torch on the same inputs.
 Tolerance: the split-bf16 3-MMA scheme carries ~2^-17 relative error per product (DESIGN.md); we require
 max|err| <= 2e-5 * (|A| @ |W|^T) element-wise scale, i.e. far below the 1e-4 output tolerance of north_star."""
 import numpy as np
@@ -133,7 +133,7 @@ def test_wgrad(M, N, K, two):
 
 
 def test_wgrad_device_row_count_masks_stale_rows():
-    """Rows >= the device-side count hold stale data (here NaN / inf): the TMA-fed producers must zero them while converting."""
+    """Rows >= the device-side count hold stale data (here NaN / inf): the producers must zero them while converting."""
     from nero_b200 import ops
     dev = torch.device('cuda')
     M, cap, N, K = 12345, 20000, 256, 256
@@ -159,9 +159,9 @@ def test_wgrad_device_row_count_masks_stale_rows():
 
 @pytest.mark.parametrize('M', [3000, 45001])
 def test_chain_matches_layerwise_and_fp64(M):
-    """Fused chain (A operand in TMEM) vs fp64 torch: 3 softplus layers with the skip-concat, then a linear head;
+    """Fused chain (A operand in shared memory) vs fp64 torch: 3 softplus layers with the skip-concat, then a linear head;
     then a derivative (DACT) chain in the reverse direction with addend / tail.  M = 45001 is 352 row tiles: every one of
-    the 148 persistent CTAs loops over at least two tiles (mbarrier phases across tiles) and the last tile is ragged."""
+    the 132 persistent CTAs loops over at least two tiles (mbarrier phases across tiles) and the last tile is ragged."""
     from nero_b200 import ops
     from nero_b200.ops import Mat, chain, chain_layer as CL
     dev = torch.device('cuda')

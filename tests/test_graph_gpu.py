@@ -1,7 +1,6 @@
 """cfg['cuda_graph']: train_step replayed from two captured CUDA graphs (nero_b200/graph.py) must produce what the eager
 kernel sequence produces on the same rays -- same ray_rgb, same losses, same parameter gradients -- without reading any
-count back to the host.  Tolerances: rgb 1e-6 (same kernels, same inputs); gradients norm-wise 1e-4 (the weight-gradient
-tiles are accumulated with L2 atomics, so the summation order differs run to run)."""
+count back to the host.  Tolerances: rgb 1e-6 (same kernels, same inputs); gradients norm-wise 1e-4."""
 import sys
 import os
 

@@ -109,7 +109,7 @@ def test_render_end_to_end_matches_oracle():
 
 
 def test_sdf_values_match_reference_1e4():
-    """SDF values of the tcgen05 MLP stack vs the fp32 reference network on random points (north_star: 1e-4)."""
+    """SDF values of the wgmma MLP stack vs the fp32 reference network on random points (north_star: 1e-4)."""
     net, g, cfg, sd = make_net('shape_bell_r32')
     gen = torch.Generator().manual_seed(5)
     x = torch.rand(4096, 3, generator=gen) * 1.6 - 0.8

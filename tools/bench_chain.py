@@ -42,5 +42,5 @@ for name, fn in cases.items():
     e1.record()
     torch.cuda.synchronize()
     us = e0.elapsed_time(e1) * 1e3 / reps
-    res[name] = {'us': round(us, 1), 'tflops': round(2.0 * M * 256 * 256 * NL / us / 1e6, 1), 'us_per_layer_tile': round(us / NL / (np.ceil(M / 128) / 148), 2)}
+    res[name] = {'us': round(us, 1), 'tflops': round(2.0 * M * 256 * 256 * NL / us / 1e6, 1), 'us_per_layer_tile': round(us / NL / (np.ceil(M / 128) / 132), 2)}
 print(json.dumps({'rows': M, 'layers': NL, 'lib': os.environ.get('NERO_LIB', 'default'), **res}))

@@ -1,4 +1,4 @@
-"""Stage II (BASELINE.json configs[3] / SURVEY.md 8d config 4: "bell material, 4096 surface samples") on one B200.
+"""Stage II (BASELINE.json configs[3] / SURVEY.md 8d config 4: "bell material, 4096 surface samples") on one H100.
 
     python tools/bench_material.py [--points 4096] [--steps 10] [--warmup 3] [--no-cpu]
 
