@@ -228,6 +228,21 @@ int nero_mc_dir_bwd(const nero_mc_params* q, void* stream);
 /* MaterialFeatsNetwork inputs (field.py:660-689): PE8 rows, skip-concat tail, xyz for the predictor input */
 int nero_mat_prep(const float* pts, int M, float* X, int ldx, float* CAT, int ldc, float* Y, int ldy, void* stream);
 
+/* ---- marching cubes (mcubes.marching_cubes in extract_geometry, network/field.py:1110-1117; extract_mesh.py) --------------
+ * u: [nx,ny,nz] fp32 C-contiguous, u[i,j,k] at index point (i,j,k); a corner is below iff u <= iso.  One vertex per grid edge
+ * (p, p+e_a) whose ends lie on different sides, at p + t e_a with t = (iso-u(p)) / (u(p+e_a)-u(p)), ordered by (linear index of
+ * p, a); triangles ordered by the linear index of their cube, then table order (nero_b200/csrc/mc_tables.cuh), wound so that
+ * cross(v1-v0, v2-v0) points to the below side.  Placement is count -> exclusive scan -> emit: the same input gives
+ * bit-identical output.  Workspaces, with nblk = ceil(nx*ny*nz / 1024): blk_cnt int[2*nblk], blk_off int64[2*nblk],
+ * totals int64[2], emap int[3*nx*ny*nz] (written at sign-change edges only; needs no initialisation).
+ * nero_mcubes_count: block counts, their scan and totals = (V, T) in device memory.
+ * nero_mcubes_emit: V, T are those totals read back by the caller; writes verts [V,3] fp32 (index space), tris [T,3] int32.
+ * Both return 1 if a dimension is < 2; emit also if V or T does not fit in int32. */
+int nero_mcubes_count(const float* u, int nx, int ny, int nz, float iso, int* blk_cnt, long long* blk_off, long long* totals,
+                      void* stream);
+int nero_mcubes_emit(const float* u, int nx, int ny, int nz, float iso, const long long* blk_off, long long V, long long T, int* emap,
+                     float* verts, int* tris, void* stream);
+
 /* sizeof() of the structures that cross this ABI, for bindings to verify their mirror layouts:
  * 0 nero_chain_layer, 1 nero_chain_params, 2 nero_mc_params, 3 finish job record, 4 prep job record. */
 int nero_abi_sizeof(int which);

@@ -151,6 +151,9 @@ int pe_standalone(const float* x, int d, int ldx, int M, int L, float scale, flo
 int ide_standalone(const float* dirs, int ldd, const float* kappa, int kstride, float kappa_scalar, int M, float* out, int ldo, cudaStream_t st);
 int occ_loss(const float* occ_prob, const float* gt, const int* sel, const int* p_ptr, int p_cap, float* loss_sum, float* docc_sign,
              cudaStream_t st);
+int mcubes_count(const float* u, int nx, int ny, int nz, float iso, int* blk_cnt, long long* blk_off, long long* totals, cudaStream_t st);
+int mcubes_emit(const float* u, int nx, int ny, int nz, float iso, const long long* blk_off, long long V, long long T, int* emap,
+                float* verts, int* tris, cudaStream_t st);
 }  // namespace nero
 
 using namespace nero;
@@ -220,6 +223,14 @@ int nero_mc_fill(const nero_mc_params* q, void* stream) { return q ? mc_fill(*q,
 int nero_mc_combine_fwd(const nero_mc_params* q, void* stream) { return q ? mc_combine_fwd(*q, (cudaStream_t)stream) : NERO_ERR_ARG; }
 int nero_mc_combine_bwd(const nero_mc_params* q, void* stream) { return q ? mc_combine_bwd(*q, (cudaStream_t)stream) : NERO_ERR_ARG; }
 int nero_mc_dir_bwd(const nero_mc_params* q, void* stream) { return q ? mc_dir_bwd(*q, (cudaStream_t)stream) : NERO_ERR_ARG; }
+int nero_mcubes_count(const float* u, int nx, int ny, int nz, float iso, int* blk_cnt, long long* blk_off, long long* totals,
+                      void* stream) {
+  return mcubes_count(u, nx, ny, nz, iso, blk_cnt, blk_off, totals, (cudaStream_t)stream);
+}
+int nero_mcubes_emit(const float* u, int nx, int ny, int nz, float iso, const long long* blk_off, long long V, long long T, int* emap,
+                     float* verts, int* tris, void* stream) {
+  return mcubes_emit(u, nx, ny, nz, iso, blk_off, V, T, emap, verts, tris, (cudaStream_t)stream);
+}
 int nero_abi_sizeof(int which) {
   switch (which) {
     case 0: return int(sizeof(nero_chain_layer));

@@ -369,15 +369,39 @@ class NeROShapeRenderer(nn.Module):
     # ------------------------------------------------------------------ geometry / material export hooks
     def extract_fields(self, bound_min=(-1.0, -1.0, -1.0), bound_max=(1.0, 1.0, 1.0), resolution=128, outside_val=1.0):
         """The SDF sampled on a regular grid, 1.0 outside the unit sphere (extract_fields, network/field.py:1090-1104); the
-        whole grid goes through the forward-only CUDA chain in one chunked query instead of 64^3 blocks."""
+        grid goes through the forward-only CUDA chain in x-slabs instead of 64^3 blocks."""
+        return self._fill_grid(bound_min, bound_max, resolution, outside_val).cpu().numpy()
+
+    GRID_SLAB_POINTS = 1 << 22
+
+    def _fill_grid(self, bound_min, bound_max, resolution, outside_val=1.0):
+        """The extract_fields grid as a device tensor [res,res,res], filled through engine.sdf_query in x-slabs of at most
+        GRID_SLAB_POINTS points (a point's value does not depend on the slab it is queried in)."""
         dev = self.deviation_network.variance.device
         axes = [torch.linspace(float(bound_min[i]), float(bound_max[i]), resolution, device=dev) for i in range(3)]
-        xx, yy, zz = torch.meshgrid(*axes, indexing='ij')
-        pts = torch.stack([xx, yy, zz], -1).reshape(-1, 3)
-        with torch.no_grad():
-            val = self.engine.sdf_query(pts)[:, 0]
-        val = torch.where(torch.norm(pts, dim=-1) >= 1.0, torch.full_like(val, float(outside_val)), val)
-        return val.reshape(resolution, resolution, resolution).cpu().numpy()
+        u = torch.empty(resolution, resolution, resolution, device=dev)
+        step = max(1, self.GRID_SLAB_POINTS // (resolution * resolution))
+        for x0 in range(0, resolution, step):
+            xx, yy, zz = torch.meshgrid(axes[0][x0:x0 + step], axes[1], axes[2], indexing='ij')
+            pts = torch.stack([xx, yy, zz], -1).reshape(-1, 3)
+            with torch.no_grad():
+                val = self.engine.sdf_query(pts)[:, 0]
+            val = torch.where(torch.norm(pts, dim=-1) >= 1.0, torch.full_like(val, float(outside_val)), val)
+            u[x0:x0 + step] = val.reshape(-1, resolution, resolution)
+        return u
+
+    def extract_mesh(self, resolution=512, threshold=0.0, bound_min=-1.0, bound_max=1.0):
+        """extract_mesh.py / extract_geometry (network/field.py:1106-1113) on the GPU: the SDF grid stays on the device and goes
+        through marching cubes (k_mcubes.cu, nero_b200.mesh).  Bounds are scalars or 3-vectors.  Returns numpy (vertices
+        float64 [V,3] in world coordinates, triangles int64 [T,3]); triangles are wound towards the inside (SDF <= threshold)."""
+        from .mesh import marching_cubes_cuda
+        bmin = np.broadcast_to(np.asarray(bound_min, np.float32), (3,))
+        bmax = np.broadcast_to(np.asarray(bound_max, np.float32), (3,))
+        u = self._fill_grid(bmin, bmax, resolution)
+        v, t = marching_cubes_cuda(u, threshold)
+        del u
+        vertices = v.cpu().numpy().astype(np.float64) / (resolution - 1.0) * (bmax - bmin)[None, :] + bmin[None, :]
+        return vertices, t.cpu().numpy().astype(np.int64)
 
     def extract_geometry(self, bound_min=(-1.0, -1.0, -1.0), bound_max=(1.0, 1.0, 1.0), resolution=128, threshold=0.0):
         """extract_geometry (network/field.py:1106-1113): marching cubes on the field; the cubes stay third party (PyMCubes,
