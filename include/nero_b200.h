@@ -243,8 +243,31 @@ int nero_mcubes_count(const float* u, int nx, int ny, int nz, float iso, int* bl
 int nero_mcubes_emit(const float* u, int nx, int ny, int nz, float iso, const long long* blk_off, long long V, long long T, int* emap,
                      float* verts, int* tris, void* stream);
 
+/* ---- relighting (the Blender Cycles render of relight.py / blender_backend/relight_backend.py) ---------------------------
+ * Path-traces one image of a triangle mesh with per-vertex NeRO materials under an equirectangular environment map
+ * (k_relight.cu; the scene is stated in nero_b200/relight.py).  One thread per pixel adds the radiance of samples
+ * [spp0, spp0 + spp) in order into accum[pixel] = (r, g, b, number of samples that hit the mesh); every random number is a
+ * hash of (seed, pixel, sample, bounce, dimension), so any split of the samples over calls gives the same bits.
+ * rays (may be NULL) receives the number of rays traced (camera + shadow + continuation).  All pointers are device pointers. */
+typedef struct nero_relight_params {
+  const void* nodes; const float* tris;           /* nero_bvh_build_host outputs (nodes, tri)                              */
+  const int* tri_ids; const int* faces;           /* [T] BVH order -> input triangle, [T,3] vertex indices                 */
+  const float* vmat;                              /* [V,8] albedo rgb, metallic, roughness (linear values), 3 unused       */
+  const float* env;                               /* [H,W,4] radiance rgb + unused, rows from the bottom (v = 0) up        */
+  const float* env_p;                             /* [H,W] probability of each texel for the light sampler                 */
+  const float* cdf_rows; const float* cdf_cols;   /* [H+1] marginal CDF over rows, [H,W+1] conditional CDF per row         */
+  float* accum;                                   /* [height*width,4] running sums                                         */
+  unsigned long long* rays;
+  float pose[12];                                 /* world -> camera [R | t], row-major, OpenCV axes (x right, y down)     */
+  float K[4];                                     /* fx, fy, cx, cy in pixels                                              */
+  int env_w, env_h, width, height;
+  int spp0, spp, max_bounces, ggx_smith;
+  unsigned int seed; int pad_;
+} nero_relight_params;
+int nero_relight_render(const nero_relight_params* q, void* stream);
+
 /* sizeof() of the structures that cross this ABI, for bindings to verify their mirror layouts:
- * 0 nero_chain_layer, 1 nero_chain_params, 2 nero_mc_params, 3 finish job record, 4 prep job record. */
+ * 0 nero_chain_layer, 1 nero_chain_params, 2 nero_mc_params, 3 finish job record, 4 prep job record, 5 nero_relight_params. */
 int nero_abi_sizeof(int which);
 
 /* nero_prep_weight for many layers in ONE launch.  jobs_dev: device array of n_jobs records

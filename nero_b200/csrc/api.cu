@@ -154,6 +154,7 @@ int occ_loss(const float* occ_prob, const float* gt, const int* sel, const int* 
 int mcubes_count(const float* u, int nx, int ny, int nz, float iso, int* blk_cnt, long long* blk_off, long long* totals, cudaStream_t st);
 int mcubes_emit(const float* u, int nx, int ny, int nz, float iso, const long long* blk_off, long long V, long long T, int* emap,
                 float* verts, int* tris, cudaStream_t st);
+int relight_render(const ::nero_relight_params& q, cudaStream_t st);
 }  // namespace nero
 
 using namespace nero;
@@ -231,6 +232,9 @@ int nero_mcubes_emit(const float* u, int nx, int ny, int nz, float iso, const lo
                      float* verts, int* tris, void* stream) {
   return mcubes_emit(u, nx, ny, nz, iso, blk_off, V, T, emap, verts, tris, (cudaStream_t)stream);
 }
+int nero_relight_render(const nero_relight_params* q, void* stream) {
+  return q ? relight_render(*q, (cudaStream_t)stream) : NERO_ERR_ARG;
+}
 int nero_abi_sizeof(int which) {
   switch (which) {
     case 0: return int(sizeof(nero_chain_layer));
@@ -238,6 +242,7 @@ int nero_abi_sizeof(int which) {
     case 2: return int(sizeof(nero_mc_params));
     case 3: return 104;   /* finish job record (k_weights.cu FinishJob) */
     case 4: return 88;    /* prep job record (k_weights.cu PrepJob) */
+    case 5: return int(sizeof(nero_relight_params));
     default: return -1;
   }
 }

@@ -9,6 +9,7 @@
 #include <cstdint>
 #include <vector>
 
+#include "bvh_traverse.cuh"
 #include "common.cuh"
 
 namespace nero {
@@ -149,55 +150,9 @@ __global__ void bvh_trace_kernel(const TraceParams q) {
   if (i >= q.n_rays) return;
   const float ox = q.org[size_t(i) * q.ldo], oy = q.org[size_t(i) * q.ldo + 1], oz = q.org[size_t(i) * q.ldo + 2];
   const float dx = q.dir[size_t(i) * q.ldd], dy = q.dir[size_t(i) * q.ldd + 1], dz = q.dir[size_t(i) * q.ldd + 2];
-  const float ix = 1.0f / dx, iy = 1.0f / dy, iz = 1.0f / dz;
-  float best = q.miss_depth;
-  int best_tri = -1;
-  int stack[48];
-  int sp = 0;
-  int node = 0;
-  const float4* n4 = reinterpret_cast<const float4*>(q.nodes);
-  while (true) {
-    const float4 a = __ldg(n4 + 2 * node), b = __ldg(n4 + 2 * node + 1);
-    // slab test against [0, best]
-    float t0 = (a.x - ox) * ix, t1 = (b.x - ox) * ix;
-    float tmin = fminf(t0, t1), tmax = fmaxf(t0, t1);
-    t0 = (a.y - oy) * iy; t1 = (b.y - oy) * iy;
-    tmin = fmaxf(tmin, fminf(t0, t1)); tmax = fminf(tmax, fmaxf(t0, t1));
-    t0 = (a.z - oz) * iz; t1 = (b.z - oz) * iz;
-    tmin = fmaxf(tmin, fminf(t0, t1)); tmax = fminf(tmax, fmaxf(t0, t1));
-    // conservative margin: a hit computed in fp32 may sit a few ulps outside the box
-    const bool overlap = (tmax >= fmaxf(tmin, 0.f) - 1e-6f * (1.0f + fabsf(tmax))) && (tmin <= best);
-    int next = -1;
-    if (overlap) {
-      const int cnt = __float_as_int(b.w), first_or_right = __float_as_int(a.w);
-      if (cnt > 0) {
-        for (int k = 0; k < cnt; ++k) {
-          const int ti = first_or_right + k;
-          const float4 v0 = __ldg(q.tris + 3 * ti), e1 = __ldg(q.tris + 3 * ti + 1), e2 = __ldg(q.tris + 3 * ti + 2);
-          // Moeller-Trumbore
-          const float px = dy * e2.z - dz * e2.y, py = dz * e2.x - dx * e2.z, pz = dx * e2.y - dy * e2.x;
-          const float det = e1.x * px + e1.y * py + e1.z * pz;
-          if (fabsf(det) > 1e-12f) {
-            const float inv = 1.0f / det;
-            const float tx = ox - v0.x, ty = oy - v0.y, tz = oz - v0.z;
-            const float u = (tx * px + ty * py + tz * pz) * inv;
-            const float qx = ty * e1.z - tz * e1.y, qy = tz * e1.x - tx * e1.z, qz = tx * e1.y - ty * e1.x;
-            const float v = (dx * qx + dy * qy + dz * qz) * inv;
-            const float t = (e2.x * qx + e2.y * qy + e2.z * qz) * inv;
-            if (u >= 0.f && v >= 0.f && u + v <= 1.f && t > 0.f && t < best) { best = t; best_tri = ti; }
-          }
-        }
-      } else {
-        stack[sp++] = first_or_right;   // right child later
-        next = node + 1;                // left child now (depth-first layout)
-      }
-    }
-    if (next < 0) {
-      if (sp == 0) break;
-      next = stack[--sp];
-    }
-    node = next;
-  }
+  const BvhHit h = bvh_traverse<false>(reinterpret_cast<const float4*>(q.nodes), q.tris, ox, oy, oz, dx, dy, dz, q.miss_depth);
+  const float best = h.t;
+  const int best_tri = h.tri;
   float nx = 0.f, ny = 0.f, nz = 0.f;
   if (best_tri >= 0) {
     const float4 e1 = __ldg(q.tris + 3 * best_tri + 1), e2 = __ldg(q.tris + 3 * best_tri + 2);
