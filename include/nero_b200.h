@@ -45,7 +45,8 @@ int nero_prep_weight(const float* v, const float* g, int K, int row0, int nrows,
  * double-backward GEMMs of SDFNetwork.gradient (field.py:155-167).
  *   mode BIAS_ACT : out = oscale * act(acc + bias)
  *   mode MUL_DACT : out[:, :ncol_main] = oscale * act'(H*hscale) * acc (+ addend);  tail[:, :] = oscale * acc[:, ncol_main:]
- *   mode TANGENT  : as MUL_DACT, plus out2 = 100 * (1 - act'(H*hscale)) * V * acc   (softplus'' term)       */
+ *   mode TANGENT  : as MUL_DACT, plus out2 = 100 * (1 - act'(H*hscale)) * V * acc   (softplus'' term)
+ * A is 16-byte aligned; H, V and addend (when given) are 8-byte aligned with even leading dimensions (else NERO_ERR_ARG). */
 int nero_linear(const float* A, int lda, int k_valid, const void* wimg, int n_pad, int k_chunks, const float* bias, int n_bias,
                 float* out, int ldo, int ncol_out, float oscale, int mode, int act, float act_param,
                 const float* H, int ldh, float hscale, int dact, const float* V, int ldv, float* out2, int ldo2,
@@ -55,7 +56,8 @@ int nero_linear(const float* A, int lda, int k_valid, const void* wimg, int n_pa
 /* ---- fused MLP chain on wgmma (A operand kept in shared memory across layers) -----------------------------------
  * Runs up to 10 consecutive layers of SDFNetwork / make_predictor / NeRFNetwork (network/field.py:130-147, 310-346,
  * 258-283) or of their gradient sweeps on each 128-row tile without writing the inter-layer activations' A operand
- * to HBM.  `chain_params_host` points to a HOST struct nero_chain_params (layout below, natural alignment). */
+ * to HBM.  `chain_params_host` points to a HOST struct nero_chain_params (layout below, natural alignment).  A0 is 16-byte
+ * aligned; every layer's H, V and addend (when given) are 8-byte aligned with even leading dimensions (else NERO_ERR_ARG). */
 typedef struct nero_chain_layer {
   const void* wimg; const float* bias;
   float* save; const float* H; const float* addend; const float* V; float* out2; float* tail;

@@ -55,15 +55,25 @@ __device__ __forceinline__ void mma_split3(float* d, uint64_t a_hi, uint64_t a_l
   Wgmma<N>::template mma<TA, TB>(d, a_hi, b_hi, 1);
 }
 
-// two adjacent fp32 values (col, col + 1) of one row; columns >= lim and rows that are not ok read as zero
+// two adjacent fp32 values (col, col + 1) (col even) of one row; columns >= lim and rows that are not ok read as zero.
+// g is 8-byte aligned and ld even (checked at launch), so at an even lim every pair is one 8-byte load; at an odd lim
+// the last pair has one column and every pair takes two 4-byte loads.  The loads are predicated rather than branched
+// around, so a caller can issue many of them before it uses the first.
+template <bool kEvenLim>
 __device__ __forceinline__ float2 ld2(const float* __restrict__ g, int ld, long row, int col, int lim, bool ok) {
-  float2 x = make_float2(0.f, 0.f);
-  if (!ok || !g || col >= lim) return x;
   const float* q = g + row * ld + col;
-  if (col + 1 < lim && (reinterpret_cast<uintptr_t>(q) & 7) == 0) return __ldg(reinterpret_cast<const float2*>(q));
-  x.x = __ldg(q);
-  if (col + 1 < lim) x.y = __ldg(q + 1);
+  float2 x = make_float2(0.f, 0.f);
+  if constexpr (kEvenLim) {
+    if (ok && col < lim) x = __ldg(reinterpret_cast<const float2*>(q));
+  } else {
+    if (ok && col < lim) x.x = __ldg(q);
+    if (ok && col + 1 < lim) x.y = __ldg(q + 1);
+  }
   return x;
+}
+// an epilogue operand pointer may be null or must allow 8-byte pair loads
+inline bool pair_aligned(const float* g, int ld) {
+  return !g || ((reinterpret_cast<uintptr_t>(g) & 7) == 0 && (ld & 1) == 0);
 }
 __device__ __forceinline__ void st2(float* __restrict__ g, int ld, long row, int col, int lim, bool ok, float a, float b) {
   if (!ok || !g || col >= lim) return;
@@ -86,11 +96,28 @@ struct EpiArgs {
   float oscale; int act; float act_param;
 };
 
-// Epilogue of accumulator columns (col, col + 1) (col even) of one row: writes out / out2 / tail as the kind defines and
-// returns the result values (those a following layer of a chain reads in the main columns).  Rows that are not ok are
-// computed with zero operands and not stored.
+// the HBM operands H, V and addend of one column pair of a derivative-product epilogue
+struct EpiIn {
+  float2 h, v, a;
+};
+template <int KIND, bool kEvenLim>
+__device__ __forceinline__ EpiIn epi_load(const EpiArgs& e, long row, int col, bool row_ok) {
+  constexpr bool kBias = (KIND == EK_BIAS_SOFTPLUS || KIND == EK_BIAS_RELU || KIND == EK_BIAS_GENERIC);
+  EpiIn in{make_float2(0.f, 0.f), make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
+  if constexpr (!kBias) {
+    const int nmain = min(e.ncol_out, e.ncol_main);
+    if constexpr (KIND != EK_DACT_NONE) in.h = ld2<kEvenLim>(e.H, e.ldh, row, col, nmain, row_ok);
+    if constexpr (KIND == EK_TANGENT) in.v = ld2<kEvenLim>(e.V, e.ldv, row, col, nmain, row_ok);
+    in.a = ld2<kEvenLim>(e.addend, e.ldadd, row, col, nmain, row_ok && e.addend);
+  }
+  return in;
+}
+
+// Epilogue of accumulator columns (col, col + 1) (col even) of one row, with its operands `in` from epi_load: writes
+// out / out2 / tail as the kind defines and returns the result values (those a following layer of a chain reads in the
+// main columns).  Rows that are not ok are computed with zero operands and not stored.
 template <int KIND>
-__device__ __forceinline__ float2 epi_pair(const EpiArgs& e, long row, int col, bool row_ok, float v0, float v1) {
+__device__ __forceinline__ float2 epi_pair(const EpiArgs& e, long row, int col, bool row_ok, float v0, float v1, const EpiIn& in) {
   constexpr bool kBias = (KIND == EK_BIAS_SOFTPLUS || KIND == EK_BIAS_RELU || KIND == EK_BIAS_GENERIC);
   const int nmain = kBias ? e.ncol_out : min(e.ncol_out, e.ncol_main);
   float r0, r1;
@@ -105,18 +132,18 @@ __device__ __forceinline__ float2 epi_pair(const EpiArgs& e, long row, int col, 
   } else {
     float s0 = 1.0f, s1 = 1.0f;
     if constexpr (KIND != EK_DACT_NONE) {
-      const float2 h = ld2(e.H, e.ldh, row, col, nmain, row_ok);
+      const float2 h = in.h;
       if constexpr (KIND == EK_DACT_RELU) { s0 = h.x > 0.0f ? 1.0f : 0.0f; s1 = h.y > 0.0f ? 1.0f : 0.0f; }
       else { s0 = dsoftplus100_fast(h.x, e.hscale); s1 = dsoftplus100_fast(h.y, e.hscale); }
     }
     r0 = e.oscale * s0 * v0;
     r1 = e.oscale * s1 * v1;
     if constexpr (KIND == EK_TANGENT) {
-      const float2 v = ld2(e.V, e.ldv, row, col, nmain, row_ok);
+      const float2 v = in.v;
       st2(e.out2, e.ldo2, row, col, nmain, row_ok, 100.0f * (1.0f - s0) * v.x * v0, 100.0f * (1.0f - s1) * v.y * v1);
     }
     if (e.addend) {
-      const float2 a = ld2(e.addend, e.ldadd, row, col, nmain, row_ok);
+      const float2 a = in.a;
       r0 += a.x;
       r1 += a.y;
     }
@@ -128,6 +155,47 @@ __device__ __forceinline__ float2 epi_pair(const EpiArgs& e, long row, int col, 
   }
   st2(e.out, e.ldo, row, col, nmain, row_ok, r0, r1);
   return make_float2(col < nmain ? r0 : 0.0f, col + 1 < nmain ? r1 : 0.0f);
+}
+
+// Column blocks (8 accumulator columns each) whose operand loads a thread issues back to back.  An epilogue that loads
+// each operand right before using it keeps one load per warp in flight and runs at a fraction of HBM bandwidth; here
+// the loads of group g + 1 are in flight while group g computes: 8 (16 with an addend) independent 8-byte loads per
+// thread, 8 in the tangent sweep, whose two operands per pair at 4 blocks would not fit the registers beside the
+// accumulators.
+template <int KIND> constexpr int kEpiGroup = KIND == EK_TANGENT ? 2 : 4;
+
+// Runs body(jb, h, row, col, row_ok, in) for every pair of this thread's accumulator fragment in column blocks jb < nb
+// (nb <= NB, a multiple of the group size) and rows row0 (h = 0) and row0 + 8 (h = 1), with `in` its epi_load operands.
+template <int KIND, int NB, class Body>
+__device__ __forceinline__ void epi_fragment(const EpiArgs& e, long row0, bool ok0, bool ok1, int lane, int nb, Body&& body) {
+  constexpr int G = NB < kEpiGroup<KIND> ? NB : kEpiGroup<KIND>;
+  static_assert(NB % G == 0, "whole groups of column blocks");
+  EpiIn in[2][2 * G];
+  const bool even_lim = (min(e.ncol_out, e.ncol_main) & 1) == 0;
+  auto load = [&](int g, EpiIn* dst) {
+    if (even_lim) {
+#pragma unroll
+      for (int j = 0; j < G; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) dst[2 * j + h] = epi_load<KIND, true>(e, row0 + 8 * h, 8 * (g * G + j) + 2 * (lane & 3), h ? ok1 : ok0);
+    } else {
+#pragma unroll
+      for (int j = 0; j < G; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) dst[2 * j + h] = epi_load<KIND, false>(e, row0 + 8 * h, 8 * (g * G + j) + 2 * (lane & 3), h ? ok1 : ok0);
+    }
+  };
+  load(0, in[0]);
+#pragma unroll
+  for (int g = 0; g < NB / G; ++g) {
+    if (g * G >= nb) break;
+    if ((g + 1) * G < nb) load(g + 1, in[(g + 1) & 1]);
+#pragma unroll
+    for (int j = 0; j < G; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        body(g * G + j, h, row0 + 8 * h, 8 * (g * G + j) + 2 * (lane & 3), h ? ok1 : ok0, in[g & 1][2 * j + h]);
+  }
 }
 
 }  // namespace nero

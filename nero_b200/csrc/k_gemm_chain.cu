@@ -52,13 +52,14 @@ constexpr uint32_t kABytes = 4 * 2 * kAPlane;       // K <= 256: four chunks x (
 constexpr uint32_t kChSmemBytes = kABytes + kWStages * kWStageBytes + 1024 /*align*/ + 64 /*barriers*/;
 static_assert(kChSmemBytes <= 232448, "shared memory budget");
 
-// columns (col, col + 1) of A row r (tile-local) as split-bf16
+// columns (col, col + 1) of A row r (tile-local) as split-bf16.  Shared-space stores: a generic store could alias the
+// epilogue's global loads as far as the compiler knows, which would keep it from issuing those loads ahead.
 __device__ __forceinline__ void put_a2(uint8_t* s_a, int r, int col, float y0, float y1) {
   uint32_t hi, lo;
   split2(y0, y1, hi, lo);
-  uint8_t* q = s_a + (col >> 6) * (2 * kAPlane) + sw128_offset(r, col & 63);
-  *reinterpret_cast<uint32_t*>(q) = hi;
-  *reinterpret_cast<uint32_t*>(q + kAPlane) = lo;
+  const uint32_t q = smem_u32(s_a) + (col >> 6) * (2 * kAPlane) + sw128_offset(r, col & 63);
+  sts_u32(q, hi);
+  sts_u32(q + kAPlane, lo);
 }
 __device__ __forceinline__ float csrc_at(const ChainLayer& L, long row, int col, bool row_ok) {
   return (L.csrc && row_ok) ? __ldg(L.csrc + row * L.ld_csrc + col) : 0.0f;
@@ -147,27 +148,18 @@ __device__ __forceinline__ void chain_layer(const ChainParams& p, const ChainLay
                   L.V, L.ldv, L.out2, L.ldo2, L.tail, L.ldt, L.ncol_out, L.ncol_main, L.oscale, L.act, L.act_param};
   const int nmain = kBias ? L.ncol_out : min(L.ncol_out, L.ncol_main);
   const int n_a = L.write_a ? max(L.a_blocks * 16, L.n_pad) : 0;       // next-A columns to define
-#pragma unroll
-  for (int hf = 0; hf < 2; ++hf) {
-    if (hf >= nh) break;
-#pragma unroll
-    for (int jb = 0; jb < HN / 8; ++jb) {
-      const int col = hf * HN + 8 * jb + 2 * (c.l & 3);
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int rl = c.wg * 64 + c.w * 16 + (c.l >> 2) + 8 * h;
-        const long row = long(tile) * CH_BM + rl;
-        const bool row_ok = rl < rows_valid;
-        float2 r = make_float2(0.f, 0.f);
-        if (col < L.ncol_out) r = epi_pair<KIND>(e, row, col, row_ok, acc[hf][4 * jb + 2 * h], acc[hf][4 * jb + 2 * h + 1]);
-        if (col < n_a) {
-          if (col >= nmain) r.x = csrc_at(L, row, col, row_ok);
-          if (col + 1 >= nmain) r.y = csrc_at(L, row, col + 1, row_ok);
-          put_a2(c.s_a, rl, col, r.x, r.y);
-        }
-      }
+  const int rl0 = c.wg * 64 + c.w * 16 + (c.l >> 2);
+  epi_fragment<KIND, 2 * HN / 8>(e, long(tile) * CH_BM + rl0, rl0 < rows_valid, rl0 + 8 < rows_valid, c.l, nh * (HN / 8),
+                                 [&](int jb, int h, long row, int col, bool row_ok, const EpiIn& in) {
+    const int hf = jb / (HN / 8), i = 4 * (jb % (HN / 8)) + 2 * h;
+    float2 r = make_float2(0.f, 0.f);
+    if (col < L.ncol_out) r = epi_pair<KIND>(e, row, col, row_ok, acc[hf][i], acc[hf][i + 1], in);
+    if (col < n_a) {
+      if (col >= nmain) r.x = csrc_at(L, row, col, row_ok);
+      if (col + 1 >= nmain) r.y = csrc_at(L, row, col + 1, row_ok);
+      put_a2(c.s_a, rl0 + 8 * h, col, r.x, r.y);
     }
-  }
+  });
   // next-A columns beyond the accumulator (skip-concat source or zero): each warp fills its own 16 rows
   const int extra = (n_a - L.n_pad) >> 1;
   for (int i = c.l; i < 16 * extra; i += 32) {
@@ -204,24 +196,27 @@ __global__ void __launch_bounds__(kChThreads, 1) gemm_chain_kernel(const __grid_
   ConsumerCtx c{s_a, s_w, full, empty, warp >> 2, warp & 3, lane, 0, threadIdx.x == 0, WCursor{int(blockIdx.x), 0, 0, 0, 0}, num_tiles};
   if (c.producer)
     for (int i = 0; i < kWStages; ++i) w_issue(p, c);
-  const int a0_cols = p.L[0].k_chunks * 64;        // every column the first layer's MMAs read (zeros beyond k_valid0)
-  const bool a0_vec = (reinterpret_cast<uintptr_t>(p.A0) & 15) == 0;
+  const int n4 = p.L[0].k_chunks * 16;     // float4 columns the first layer's MMAs read (zeros beyond k_valid0)
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     const int rows_valid = min(CH_BM, M - tile * CH_BM);
-    // ---- first A operand: fp32 rows from HBM -> split-bf16; each warp converts its own 16 rows
+    // ---- first A operand: fp32 rows from HBM -> split-bf16; each warp converts its own 16 rows, 16 * n4 float4 = 8 per
+    // lane and K chunk, in batches of 4 whose loads are all issued before the first conversion
     {
-      const int n4 = a0_cols / 4;
-      for (int i = lane; i < 16 * n4; i += 32) {
-        const int rl = c.wg * 64 + c.w * 16 + i / n4, col = 4 * (i % n4);
-        const long row = long(tile) * CH_BM + rl;
-        float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (rl < rows_valid && col < p.k_valid0) {
-          const float* q = p.A0 + row * p.lda0 + col;
-          if (a0_vec) x = __ldg(reinterpret_cast<const float4*>(q));      // k_valid0 and lda0 are multiples of 4
-          else { x.x = __ldg(q); x.y = __ldg(q + 1); x.z = __ldg(q + 2); x.w = __ldg(q + 3); }
+      for (int b = 0; b < 2 * p.L[0].k_chunks; ++b) {
+        float4 x[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          const int i = lane + 32 * (4 * b + u), rl = c.wg * 64 + c.w * 16 + i / n4, col = 4 * (i % n4);
+          const float* q = p.A0 + (long(tile) * CH_BM + rl) * p.lda0 + col;    // 16-byte aligned: checked at launch
+          x[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+          if (rl < rows_valid && col < p.k_valid0) x[u] = __ldg(reinterpret_cast<const float4*>(q));
         }
-        put_a2(s_a, rl, col, x.x, x.y);
-        put_a2(s_a, rl, col + 2, x.z, x.w);
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          const int i = lane + 32 * (4 * b + u), rl = c.wg * 64 + c.w * 16 + i / n4, col = 4 * (i % n4);
+          put_a2(s_a, rl, col, x[u].x, x[u].y);
+          put_a2(s_a, rl, col + 2, x[u].z, x[u].w);
+        }
       }
       fence_proxy_async_smem();
       named_bar(1 + c.wg, 128);
@@ -245,10 +240,13 @@ __global__ void __launch_bounds__(kChThreads, 1) gemm_chain_kernel(const __grid_
 
 // ---------------------------------------------------------------------------------------------- host side
 int chain_dispatch(const ChainParams& p, cudaStream_t stream) {
-  if (p.n_layers <= 0 || p.n_layers > kMaxChainLayers || (p.lda0 & 3) || (p.k_valid0 & 3) || p.k_valid0 > 256 || !p.A0) return NERO_ERR_ARG;
+  if (p.n_layers <= 0 || p.n_layers > kMaxChainLayers || (p.lda0 & 3) || (p.k_valid0 & 3) || p.k_valid0 > 256 || !p.A0 ||
+      (reinterpret_cast<uintptr_t>(p.A0) & 15))
+    return NERO_ERR_ARG;
   for (int l = 0; l < p.n_layers; ++l) {
     const ChainLayer& L = p.L[l];
     if (L.n_pad % 16 || L.n_pad < 16 || L.n_pad > 256) return NERO_ERR_ARG;
+    if (!pair_aligned(L.H, L.ldh) || !pair_aligned(L.V, L.ldv) || !pair_aligned(L.addend, L.ldadd)) return NERO_ERR_ARG;
     if (L.k_chunks < 1 || L.k_chunks > 4 || L.ncol_out > L.n_pad || !L.wimg) return NERO_ERR_ARG;
     if (L.write_a && (L.a_blocks > 16 || (l + 1 < p.n_layers && L.a_blocks < 4 * p.L[l + 1].k_chunks))) return NERO_ERR_ARG;
     if (L.kind == EK_TANGENT && (!L.H || !L.V || !L.out2)) return NERO_ERR_ARG;

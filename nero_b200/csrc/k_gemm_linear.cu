@@ -112,15 +112,11 @@ __global__ void __launch_bounds__(kLinearThreads, 1) gemm_linear_kernel(const Li
     }
     wgmma_wait<0>();
     fence_regs<NPAD / 2>(acc);
-#pragma unroll
-    for (int jb = 0; jb < NPAD / 8; ++jb) {
-      const int col = 8 * jb + 2 * (l & 3);
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const long row = long(tile) * BM + wg * 64 + w * 16 + (l >> 2) + 8 * h;
-        if (row < M && col < p.ncol_out) epi_pair<EPI>(e, row, col, true, acc[4 * jb + 2 * h], acc[4 * jb + 2 * h + 1]);
-      }
-    }
+    const long row0 = long(tile) * BM + wg * 64 + w * 16 + (l >> 2);
+    epi_fragment<EPI, NPAD / 8>(e, row0, row0 < M, row0 + 8 < M, l, NPAD / 8,
+                                [&](int jb, int h, long row, int col, bool row_ok, const EpiIn& in) {
+      if (row_ok && col < p.ncol_out) epi_pair<EPI>(e, row, col, true, acc[4 * jb + 2 * h], acc[4 * jb + 2 * h + 1], in);
+    });
   }
 }
 
@@ -158,6 +154,7 @@ int linear_dispatch(const LinearParams& p, cudaStream_t stream) {
   if (p.k_chunks <= 0 || (p.k_valid & 3) || (p.lda & 3) || (reinterpret_cast<uintptr_t>(p.A) & 15)) return NERO_ERR_ARG;
   if (p.mode == EPI_TANGENT && (!p.H || !p.V || !p.out2 || p.dact != ACT_SOFTPLUS100)) return NERO_ERR_ARG;
   if (p.mode == EPI_MUL_DACT && p.dact != ACT_NONE && !p.H) return NERO_ERR_ARG;
+  if (!pair_aligned(p.H, p.ldh) || !pair_aligned(p.V, p.ldv) || !pair_aligned(p.addend, p.ldadd)) return NERO_ERR_ARG;
   switch (p.n_pad) {
     case 16: return dispatch_epi<16>(p, stream);
     case 64: return dispatch_epi<64>(p, stream);
