@@ -268,8 +268,43 @@ typedef struct nero_relight_params {
 } nero_relight_params;
 int nero_relight_render(const nero_relight_params* q, void* stream);
 
+/* ---- shape evaluation (eval_synthetic_shape.py / eval_real_shape.py; the protocol is stated in nero_b200/evaluate.py) ------
+ * nero_depth_render: depth map of a triangle mesh as the reference's nvdiffrast call produces it (w = 1): per pixel (x, y) the
+ * closest hit of the ray through (x + 1/2, y + 1/2), depth = sum b_i z_i^2 / sum b_i z_i from its 3-D barycentrics b and the
+ * camera depths z of the input vertices; 0 on a miss or outside [near_z, far_z].  K must have zero skew and last row (0, 0, 1). */
+typedef struct nero_depth_params {
+  const void* nodes; const float* tris;           /* nero_bvh_build_host outputs (nodes, tri)                              */
+  const int* tri_ids; const int* faces;           /* [T] BVH order -> input triangle, [T,3] vertex indices                 */
+  const float* verts;                             /* [V,3]                                                                 */
+  float* depth;                                   /* [height,width] output                                                 */
+  float pose[12];                                 /* world -> camera [R | t], row-major, OpenCV axes (x right, y down)     */
+  float K[9];                                     /* 3x3 row-major intrinsics in pixels                                    */
+  int width, height;
+  float near_z, far_z;
+} nero_depth_params;
+int nero_depth_render(const nero_depth_params* q, void* stream);
+/* Ordered compaction of the pixels with lo < depth < hi of n_views stacked [height,width] depth maps, in (view, row, column)
+ * order, each unprojected at its integer pixel coordinates, X_cam = d ((x - cx)/fx, (y - cy)/fy, 1), and moved to world
+ * space, X = R_c2w X_cam + c, in fp64; written as fp32 pts [n,3].  cams: [n_views,16] fp64 = R_c2w (row-major 3x3), camera
+ * centre c, fx, fy, cx, cy.  Count -> exclusive scan -> emit; workspaces with nblk = ceil(n_views*height*width / 1024):
+ * blk_cnt int[nblk], blk_off int64[nblk], total int64[1].  emit takes n = *total read back by the caller. */
+int nero_depth_points_count(const float* depth, int n_views, int height, int width, float lo, float hi, int* blk_cnt,
+                            long long* blk_off, long long* total, void* stream);
+int nero_depth_points_emit(const float* depth, int n_views, int height, int width, float lo, float hi, const double* cams,
+                           const long long* blk_off, long long n, float* pts, void* stream);
+/* Open3D VoxelDownSample in fp64.  nero_voxel_keys: key = i << 42 | j << 21 | k with (i, j, k) = floor((p - min) / voxel);
+ * bounds_host (HOST) = (min_x, min_y, min_z, max_x, max_y, max_z) with min = the cloud's minimum - voxel/2; returns 1 if an
+ * index along any axis can reach 2^21.  nero_voxel_mean: given order = a stable key sort of the points and ends = inclusive
+ * cumulative counts of the m distinct keys, out[v] = mean of the points of voxel v, summed in input order. */
+int nero_voxel_keys(const double* pts, long long n, const double* bounds_host, double voxel, long long* keys, void* stream);
+int nero_voxel_mean(const double* pts, const long long* order, const long long* ends, long long m, double* out, void* stream);
+/* dist[i] = min_j |q_i - t_j| over t [m,3] (m >= 1), q [n,3], fp32: ((dx*dx + dy*dy) + dz*dz) rounded to nearest without
+ * contraction, minimum, correctly rounded square root.  The result does not depend on the launch shape. */
+int nero_nearest_dist(const float* q, long long n, const float* t, long long m, float* dist, void* stream);
+
 /* sizeof() of the structures that cross this ABI, for bindings to verify their mirror layouts:
- * 0 nero_chain_layer, 1 nero_chain_params, 2 nero_mc_params, 3 finish job record, 4 prep job record, 5 nero_relight_params. */
+ * 0 nero_chain_layer, 1 nero_chain_params, 2 nero_mc_params, 3 finish job record, 4 prep job record, 5 nero_relight_params,
+ * 6 nero_depth_params. */
 int nero_abi_sizeof(int which);
 
 /* nero_prep_weight for many layers in ONE launch.  jobs_dev: device array of n_jobs records

@@ -155,6 +155,14 @@ int mcubes_count(const float* u, int nx, int ny, int nz, float iso, int* blk_cnt
 int mcubes_emit(const float* u, int nx, int ny, int nz, float iso, const long long* blk_off, long long V, long long T, int* emap,
                 float* verts, int* tris, cudaStream_t st);
 int relight_render(const ::nero_relight_params& q, cudaStream_t st);
+int depth_render(const ::nero_depth_params& q, cudaStream_t st);
+int depth_points_count(const float* depth, int n_views, int height, int width, float lo, float hi, int* blk_cnt, long long* blk_off,
+                       long long* total, cudaStream_t st);
+int depth_points_emit(const float* depth, int n_views, int height, int width, float lo, float hi, const double* cams,
+                      const long long* blk_off, long long n, float* pts, cudaStream_t st);
+int voxel_keys(const double* pts, long long n, const double* bounds, double voxel, long long* keys, cudaStream_t st);
+int voxel_mean(const double* pts, const long long* order, const long long* ends, long long m, double* out, cudaStream_t st);
+int nearest_dist(const float* q, long long n, const float* t, long long m, float* dist, cudaStream_t st);
 }  // namespace nero
 
 using namespace nero;
@@ -235,6 +243,24 @@ int nero_mcubes_emit(const float* u, int nx, int ny, int nz, float iso, const lo
 int nero_relight_render(const nero_relight_params* q, void* stream) {
   return q ? relight_render(*q, (cudaStream_t)stream) : NERO_ERR_ARG;
 }
+int nero_depth_render(const nero_depth_params* q, void* stream) { return q ? depth_render(*q, (cudaStream_t)stream) : NERO_ERR_ARG; }
+int nero_depth_points_count(const float* depth, int n_views, int height, int width, float lo, float hi, int* blk_cnt,
+                            long long* blk_off, long long* total, void* stream) {
+  return depth_points_count(depth, n_views, height, width, lo, hi, blk_cnt, blk_off, total, (cudaStream_t)stream);
+}
+int nero_depth_points_emit(const float* depth, int n_views, int height, int width, float lo, float hi, const double* cams,
+                           const long long* blk_off, long long n, float* pts, void* stream) {
+  return depth_points_emit(depth, n_views, height, width, lo, hi, cams, blk_off, n, pts, (cudaStream_t)stream);
+}
+int nero_voxel_keys(const double* pts, long long n, const double* bounds_host, double voxel, long long* keys, void* stream) {
+  return voxel_keys(pts, n, bounds_host, voxel, keys, (cudaStream_t)stream);
+}
+int nero_voxel_mean(const double* pts, const long long* order, const long long* ends, long long m, double* out, void* stream) {
+  return voxel_mean(pts, order, ends, m, out, (cudaStream_t)stream);
+}
+int nero_nearest_dist(const float* q, long long n, const float* t, long long m, float* dist, void* stream) {
+  return nearest_dist(q, n, t, m, dist, (cudaStream_t)stream);
+}
 int nero_abi_sizeof(int which) {
   switch (which) {
     case 0: return int(sizeof(nero_chain_layer));
@@ -243,6 +269,7 @@ int nero_abi_sizeof(int which) {
     case 3: return 104;   /* finish job record (k_weights.cu FinishJob) */
     case 4: return 88;    /* prep job record (k_weights.cu PrepJob) */
     case 5: return int(sizeof(nero_relight_params));
+    case 6: return int(sizeof(nero_depth_params));
     default: return -1;
   }
 }
