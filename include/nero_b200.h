@@ -64,8 +64,8 @@ typedef struct nero_chain_layer {
   int n_pad, k_chunks, n_bias, ncol_out, ncol_main, kind, act;   /* kind: 0 bias+softplus100, 1 bias+relu, 2 bias+act(generic), */
   int ld_save, ldh, ldadd, ldv, ldo2, ldt;                        /*       3 dsoftplus*acc, 4 drelu*acc, 5 acc, 6 tangent        */
   float oscale, hscale, act_param;
-  int write_a, a_blocks;
-  const float* csrc; int ld_csrc;
+  int write_a, a_blocks;      /* write_a: the output becomes the next A operand; a_blocks: 16-col blocks of it to define */
+  const float* csrc; int ld_csrc;   /* skip-concat source: columns >= ncol_out of the next A operand come from csrc[row, col] */
   int pad_;
 } nero_chain_layer;
 typedef struct nero_chain_params {
@@ -302,20 +302,28 @@ int nero_voxel_mean(const double* pts, const long long* order, const long long* 
  * contraction, minimum, correctly rounded square root.  The result does not depend on the launch shape. */
 int nero_nearest_dist(const float* q, long long n, const float* t, long long m, float* dist, void* stream);
 
-/* sizeof() of the structures that cross this ABI, for bindings to verify their mirror layouts:
- * 0 nero_chain_layer, 1 nero_chain_params, 2 nero_mc_params, 3 finish job record, 4 prep job record, 5 nero_relight_params,
+/* sizeof() of the structures that cross this ABI, for bindings to verify their layouts against the library:
+ * 0 nero_chain_layer, 1 nero_chain_params, 2 nero_mc_params, 3 nero_finish_job, 4 nero_prep_job, 5 nero_relight_params,
  * 6 nero_depth_params. */
 int nero_abi_sizeof(int which);
 
-/* nero_prep_weight for many layers in ONE launch.  jobs_dev: device array of n_jobs records
- *   { const float* v, *g; const int* kmap; void* img_f, *img_t; float* w_eff;
- *     int K, row0, nrows, rows_pad_f, rows_pad_t, t_c0, t_ncols, ld_weff; float in_scale; int pad; }   (88 bytes each) */
+/* nero_prep_weight for many layers in ONE launch.  jobs_dev: device array of n_jobs records (same meaning as the
+ * nero_prep_weight arguments). */
+typedef struct nero_prep_job {
+  const float* v; const float* g; const int* kmap; void* img_f; void* img_t; float* w_eff;
+  int K, row0, nrows, rows_pad_f, rows_pad_t, t_c0, t_ncols, ld_weff;
+  float in_scale; int pad_;
+} nero_prep_job;
 int nero_prep_weight_batch(const void* jobs_dev, int n_jobs, int max_rows, void* stream);
 
-/* nero_wgrad_finish for many layers in ONE launch.  jobs_dev: device array of n_jobs records
- *   { const float* partial, *bias_partial; const int* kmap; const float* v, *g; float* grad_w, *grad_g, *grad_b;
- *     const float* extra_row; int P, rows_partial, ld_partial, K, row0, nrows; float in_scale, extra_scale; }
- * (same meaning as the nero_wgrad_finish arguments; 104 bytes each).  Jobs of one launch must not share destination rows. */
+/* nero_wgrad_finish for many layers in ONE launch.  jobs_dev: device array of n_jobs records (same meaning as the
+ * nero_wgrad_finish arguments).  Jobs of one launch must not share destination rows. */
+typedef struct nero_finish_job {
+  const float* partial; const float* bias_partial; const int* kmap; const float* v; const float* g;
+  float* grad_w; float* grad_g; float* grad_b; const float* extra_row;
+  int P, rows_partial, ld_partial, K, row0, nrows;
+  float in_scale, extra_scale;
+} nero_finish_job;
 int nero_wgrad_finish_batch(const void* jobs_dev, int n_jobs, int max_rows, int max_k, void* stream);
 
 /* Adam step over one flat fp32 parameter buffer (torch.optim.Adam semantics; replaces the multi-tensor optimizer launch of

@@ -9,7 +9,9 @@ CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libnero_b200.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
-FLAGS = ARCH + ['-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC',
+# diagnostic 338 (two declarations of one extern "C" function with different parameters) is only a warning for a
+# definition inside a namespace; as an error it makes every entry point compile against its prototype in the header
+FLAGS = ARCH + ['-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC', '--diag-error', '338',
          '--expt-relaxed-constexpr', '-Xptxas', '-v' if os.environ.get('NERO_PTXAS_V') else '-O3']
 
 

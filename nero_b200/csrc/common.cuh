@@ -5,6 +5,10 @@
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 
+// Every k_*.cu defines the entry points of its kernels against these prototypes, inside extern "C": a definition whose
+// parameters differ from its declaration does not compile.
+#include "../../include/nero_b200.h"
+
 #if defined(__CUDACC__)
 #define NERO_HD __host__ __device__ __forceinline__
 #else

@@ -105,7 +105,9 @@ struct Builder {
 
 // Host build.  verts [V,3] fp32, tris [T,3] int32 (host memory).  Outputs (host memory, caller-allocated):
 //   nodes_out  [2T] x 32 B, tri_out [T] x 3 float4 (v0, e1, e2; w unused), tri_id_out [T] original triangle index.
-int bvh_build_host(const float* verts, int V, const int* tris, int T, void* nodes_out, float* tri_out, int* tri_id_out, int* n_nodes) {
+extern "C" int nero_bvh_build_host(const float* verts, int V, const int* tris, int T, void* nodes_out, float* tri_out, int* tri_id_out,
+                                   int* n_nodes) {
+  if (!verts || !tris || !nodes_out || !tri_out || !tri_id_out || !n_nodes) return NERO_ERR_ARG;
   if (T <= 0 || V <= 0) return NERO_ERR_ARG;
   std::vector<BuildTri> t(T);
   for (int i = 0; i < T; ++i) {
@@ -164,9 +166,13 @@ __global__ void bvh_trace_kernel(const TraceParams q) {
   q.nrm_hit[i] = make_float4(nx, ny, nz, best_tri >= 0 ? 1.0f : 0.0f);
 }
 
-int bvh_trace(const TraceParams& q, cudaStream_t st) {
-  if (q.n_rays <= 0) return NERO_OK;
-  bvh_trace_kernel<<<(q.n_rays + 127) / 128, 128, 0, st>>>(q);
+extern "C" int nero_bvh_trace(const void* nodes, const float* tris, int n_rays, const float* org, int ldo, const float* dir, int ldd,
+                              float* pos_depth, float* nrm_hit, float miss_depth, int flip, void* stream) {
+  if (!nodes || !tris || (n_rays > 0 && (!org || !dir || !pos_depth || !nrm_hit))) return NERO_ERR_ARG;
+  if (n_rays <= 0) return NERO_OK;
+  const TraceParams q{reinterpret_cast<const BvhNode*>(nodes), reinterpret_cast<const float4*>(tris), n_rays, org, ldo, dir, ldd,
+                      reinterpret_cast<float4*>(pos_depth), reinterpret_cast<float4*>(nrm_hit), miss_depth, flip};
+  bvh_trace_kernel<<<(n_rays + 127) / 128, 128, 0, (cudaStream_t)stream>>>(q);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }

@@ -36,12 +36,13 @@ __global__ void __launch_bounds__(kEncBlock) pe_kernel(const float* __restrict__
   }
 }
 
-int pe_standalone(const float* x, int d, int ldx, int M, int L, float scale, float* out, int ldo, cudaStream_t st) {
+extern "C" int nero_pe(const float* x, int d, int ldx, int M, int L, float scale, float* out, int ldo, void* stream) {
   if (!x || !out || (d != 3 && d != 4) || L < 0 || L > 16 || ldx < d || ldo < d * (1 + 2 * L)) return NERO_ERR_ARG;
   if (M <= 0) return NERO_OK;
   const int ncol = d * (1 + 2 * L);
   const size_t smem = size_t(kEncBlock) * (ncol | 1) * sizeof(float);
   const int grid = (M + kEncBlock - 1) / kEncBlock;
+  const cudaStream_t st = (cudaStream_t)stream;
   if (d == 3) pe_kernel<3><<<grid, kEncBlock, smem, st>>>(x, ldx, M, L, scale, out, ldo);
   else {
     static bool attr = false;

@@ -12,7 +12,6 @@
 //                 squared distance ((dx*dx + dy*dy) + dz*dz) with round-to-nearest, uncontracted operations.
 //
 // Nothing here uses atomics to place or combine values, so every output is bit-identical from run to run.
-#include "../../include/nero_b200.h"
 #include "bvh_traverse.cuh"
 #include "common.cuh"
 
@@ -248,20 +247,25 @@ bool ev_grid(int n_views, int height, int width, long long& N, int& nblk) {
 
 }  // namespace
 
-int depth_render(const nero_depth_params& q, cudaStream_t st) {
+extern "C" {
+
+int nero_depth_render(const nero_depth_params* p, void* stream) {
+  if (!p) return NERO_ERR_ARG;
+  const nero_depth_params& q = *p;
   if (!q.nodes || !q.tris || !q.tri_ids || !q.faces || !q.verts || !q.depth || q.width < 1 || q.height < 1) return NERO_ERR_ARG;
   // pinhole intrinsics only: zero skew, last row (0, 0, 1), non-zero focal lengths
   if (q.K[1] != 0.f || q.K[3] != 0.f || q.K[6] != 0.f || q.K[7] != 0.f || q.K[8] != 1.f || q.K[0] == 0.f || q.K[4] == 0.f)
     return NERO_ERR_ARG;
   if (!(q.near_z < q.far_z)) return NERO_ERR_ARG;
   const dim3 grid((q.width + 15) / 16, (q.height + 7) / 8);
-  depth_render_kernel<<<grid, 128, 0, st>>>(q);
+  depth_render_kernel<<<grid, 128, 0, (cudaStream_t)stream>>>(q);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
 
-int depth_points_count(const float* depth, int n_views, int height, int width, float lo, float hi, int* blk_cnt, long long* blk_off,
-                       long long* total, cudaStream_t st) {
+int nero_depth_points_count(const float* depth, int n_views, int height, int width, float lo, float hi, int* blk_cnt,
+                            long long* blk_off, long long* total, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
   long long N;
   int nblk;
   if (!depth || !blk_cnt || !blk_off || !total || !ev_grid(n_views, height, width, N, nblk)) return NERO_ERR_ARG;
@@ -271,19 +275,19 @@ int depth_points_count(const float* depth, int n_views, int height, int width, f
   return NERO_OK;
 }
 
-int depth_points_emit(const float* depth, int n_views, int height, int width, float lo, float hi, const double* cams,
-                      const long long* blk_off, long long n, float* pts, cudaStream_t st) {
+int nero_depth_points_emit(const float* depth, int n_views, int height, int width, float lo, float hi, const double* cams,
+                           const long long* blk_off, long long n, float* pts, void* stream) {
   long long N;
   int nblk;
   if (!depth || !cams || !blk_off || n < 0 || !ev_grid(n_views, height, width, N, nblk) || n > N) return NERO_ERR_ARG;
   if (n == 0) return NERO_OK;
   if (!pts) return NERO_ERR_ARG;
-  points_emit_kernel<<<nblk, kEvThreads, 0, st>>>(depth, N, (long long)height * width, width, lo, hi, cams, blk_off, pts);
+  points_emit_kernel<<<nblk, kEvThreads, 0, (cudaStream_t)stream>>>(depth, N, (long long)height * width, width, lo, hi, cams, blk_off, pts);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
 
-int voxel_keys(const double* pts, long long n, const double* bounds, double voxel, long long* keys, cudaStream_t st) {
+int nero_voxel_keys(const double* pts, long long n, const double* bounds, double voxel, long long* keys, void* stream) {
   if (!bounds || n < 0 || !(voxel > 0.0) || (n > 0 && (!pts || !keys))) return NERO_ERR_ARG;
   for (int a = 0; a < 3; ++a) {
     // the largest index along each axis, computed as the kernel computes it, must fit 21 bits
@@ -291,27 +295,29 @@ int voxel_keys(const double* pts, long long n, const double* bounds, double voxe
     if (!(bounds[a] <= bounds[3 + a]) || !(hi < double(kVoxMax))) return NERO_ERR_ARG;
   }
   if (n == 0) return NERO_OK;
-  voxel_keys_kernel<<<unsigned((n + 255) / 256), 256, 0, st>>>(pts, n, bounds[0], bounds[1], bounds[2], voxel, keys);
+  voxel_keys_kernel<<<unsigned((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(pts, n, bounds[0], bounds[1], bounds[2], voxel, keys);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
 
-int voxel_mean(const double* pts, const long long* order, const long long* ends, long long m, double* out, cudaStream_t st) {
+int nero_voxel_mean(const double* pts, const long long* order, const long long* ends, long long m, double* out, void* stream) {
   if (m < 0 || (m > 0 && (!pts || !order || !ends || !out))) return NERO_ERR_ARG;
   if (m == 0) return NERO_OK;
-  voxel_mean_kernel<<<unsigned((m + 255) / 256), 256, 0, st>>>(pts, order, ends, m, out);
+  voxel_mean_kernel<<<unsigned((m + 255) / 256), 256, 0, (cudaStream_t)stream>>>(pts, order, ends, m, out);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
 
-int nearest_dist(const float* q, long long n, const float* t, long long m, float* dist, cudaStream_t st) {
+int nero_nearest_dist(const float* q, long long n, const float* t, long long m, float* dist, void* stream) {
   if (n < 0 || m < 1 || !t || (n > 0 && (!q || !dist))) return NERO_ERR_ARG;
   if (n == 0) return NERO_OK;
   const long long nb = (n + kNnThreads * kNnQ - 1) / (kNnThreads * kNnQ);
   if (nb > 0x7fffffffLL) return NERO_ERR_ARG;
-  nearest_kernel<<<unsigned(nb), kNnThreads, 0, st>>>(q, n, t, m, dist);
+  nearest_kernel<<<unsigned(nb), kNnThreads, 0, (cudaStream_t)stream>>>(q, n, t, m, dist);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
+
+}  // extern "C"
 
 }  // namespace nero

@@ -22,23 +22,7 @@
 namespace nero {
 
 constexpr int kMaxChainLayers = 10;
-
-// ---------------------------------------------------------------------------------------------- C ABI (host) structs
-struct ChainLayer {
-  const uint8_t* wimg; const float* bias;
-  float* save; const float* H; const float* addend; const float* V; float* out2; float* tail;
-  int n_pad, k_chunks, n_bias, ncol_out, ncol_main, kind, act;
-  int ld_save, ldh, ldadd, ldv, ldo2, ldt;
-  float oscale, hscale, act_param;
-  int write_a, a_blocks;      // write_a: the output becomes the next A operand; a_blocks: 16-col blocks of it to define
-  const float* csrc; int ld_csrc;   // skip-concat source: columns >= ncol_out of the next A operand come from csrc[row, col]
-  int pad_;
-};
-struct ChainParams {
-  const float* A0; int lda0; int k_valid0;
-  int n_layers; const int* m_ptr; int m_cap;
-  ChainLayer L[kMaxChainLayers];
-};
+static_assert(sizeof(nero_chain_params::L) / sizeof(nero_chain_layer) == kMaxChainLayers, "the C ABI's nero_chain_params.L length");
 
 // ---------------------------------------------------------------------------------------------- configuration
 constexpr int CH_BM = 128;
@@ -61,7 +45,7 @@ __device__ __forceinline__ void put_a2(uint8_t* s_a, int r, int col, float y0, f
   sts_u32(q, hi);
   sts_u32(q + kAPlane, lo);
 }
-__device__ __forceinline__ float csrc_at(const ChainLayer& L, long row, int col, bool row_ok) {
+__device__ __forceinline__ float csrc_at(const nero_chain_layer& L, long row, int col, bool row_ok) {
   return (L.csrc && row_ok) ? __ldg(L.csrc + row * L.ld_csrc + col) : 0.0f;
 }
 
@@ -79,17 +63,17 @@ struct ConsumerCtx {
 };
 
 // load the next weight stage into its ring slot once both warpgroups have released the slot's previous contents
-__device__ __forceinline__ void w_issue(const ChainParams& p, ConsumerCtx& c) {
+__device__ __forceinline__ void w_issue(const nero_chain_params& p, ConsumerCtx& c) {
   WCursor& q = c.q;
   if (q.tile >= c.num_tiles) return;
-  const ChainLayer& L = p.L[q.li];
+  const nero_chain_layer& L = p.L[q.li];
   const int nh = L.n_pad > HN ? 2 : 1;
   const uint32_t plane = uint32_t(L.n_pad) * 128u;
   const int s = q.g % kWStages;
   mbar_wait(&c.empty[s], ((q.g / kWStages) & 1) ^ 1);
   // rows [hf*128, +rows) of the chunk's hi plane and of its lo plane; stage rows beyond them only feed unused columns
   const uint32_t bytes = min(kHalfBytes, plane - q.hf * kHalfBytes);
-  const uint8_t* src = L.wimg + size_t(q.kc) * 2u * plane + size_t(q.hf) * kHalfBytes;
+  const uint8_t* src = static_cast<const uint8_t*>(L.wimg) + size_t(q.kc) * 2u * plane + size_t(q.hf) * kHalfBytes;
   mbar_arrive_expect_tx(&c.full[s], 2u * bytes);
   bulk_copy_g2s(c.s_w + s * kWStageBytes, src, bytes, &c.full[s]);
   bulk_copy_g2s(c.s_w + s * kWStageBytes + kHalfBytes, src + plane, bytes, &c.full[s]);
@@ -103,7 +87,7 @@ __device__ __forceinline__ void w_issue(const ChainParams& p, ConsumerCtx& c) {
   }
 }
 // this warp is done with weight stage s (its MMAs reading it have completed)
-__device__ __forceinline__ void w_release(const ChainParams& p, ConsumerCtx& c, int s) {
+__device__ __forceinline__ void w_release(const nero_chain_params& p, ConsumerCtx& c, int s) {
   if (c.l == 0) mbar_arrive(&c.empty[s]);
   if (c.producer) w_issue(p, c);
   __syncwarp();
@@ -111,7 +95,8 @@ __device__ __forceinline__ void w_release(const ChainParams& p, ConsumerCtx& c, 
 
 // the MMAs of one layer followed by its epilogue, for this thread's warpgroup
 template <int KIND>
-__device__ __forceinline__ void chain_layer(const ChainParams& p, const ChainLayer& L, ConsumerCtx& c, int tile, int rows_valid) {
+__device__ __forceinline__ void chain_layer(const nero_chain_params& p, const nero_chain_layer& L, ConsumerCtx& c, int tile,
+                                            int rows_valid) {
   constexpr bool kBias = (KIND == EK_BIAS_SOFTPLUS || KIND == EK_BIAS_RELU || KIND == EK_BIAS_GENERIC);
   const int nh = L.n_pad > HN ? 2 : 1;
   float acc[2][HN / 2];
@@ -175,7 +160,7 @@ __device__ __forceinline__ void chain_layer(const ChainParams& p, const ChainLay
 // FAM: 0 = bias/activation epilogues (forward chains), 1 = derivative-product epilogues (gradient sweeps), 2 = tangent
 // sweep.  One instantiation per family keeps the code of each kernel small.
 template <int FAM>
-__global__ void __launch_bounds__(kChThreads, 1) gemm_chain_kernel(const __grid_constant__ ChainParams p) {
+__global__ void __launch_bounds__(kChThreads, 1) gemm_chain_kernel(const __grid_constant__ nero_chain_params p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* s_a = smem;
@@ -222,7 +207,7 @@ __global__ void __launch_bounds__(kChThreads, 1) gemm_chain_kernel(const __grid_
       named_bar(1 + c.wg, 128);
     }
     for (int li = 0; li < p.n_layers; ++li) {
-      const ChainLayer& L = p.L[li];
+      const nero_chain_layer& L = p.L[li];
       if constexpr (FAM == 0) {
         if (L.kind == EK_BIAS_SOFTPLUS) chain_layer<EK_BIAS_SOFTPLUS>(p, L, c, tile, rows_valid);
         else if (L.kind == EK_BIAS_RELU) chain_layer<EK_BIAS_RELU>(p, L, c, tile, rows_valid);
@@ -239,12 +224,14 @@ __global__ void __launch_bounds__(kChThreads, 1) gemm_chain_kernel(const __grid_
 }
 
 // ---------------------------------------------------------------------------------------------- host side
-int chain_dispatch(const ChainParams& p, cudaStream_t stream) {
+extern "C" int nero_chain(const void* chain_params_host, void* stream) {
+  if (!chain_params_host) return NERO_ERR_ARG;
+  const nero_chain_params& p = *static_cast<const nero_chain_params*>(chain_params_host);
   if (p.n_layers <= 0 || p.n_layers > kMaxChainLayers || (p.lda0 & 3) || (p.k_valid0 & 3) || p.k_valid0 > 256 || !p.A0 ||
       (reinterpret_cast<uintptr_t>(p.A0) & 15))
     return NERO_ERR_ARG;
   for (int l = 0; l < p.n_layers; ++l) {
-    const ChainLayer& L = p.L[l];
+    const nero_chain_layer& L = p.L[l];
     if (L.n_pad % 16 || L.n_pad < 16 || L.n_pad > 256) return NERO_ERR_ARG;
     if (!pair_aligned(L.H, L.ldh) || !pair_aligned(L.V, L.ldv) || !pair_aligned(L.addend, L.ldadd)) return NERO_ERR_ARG;
     if (L.k_chunks < 1 || L.k_chunks > 4 || L.ncol_out > L.n_pad || !L.wimg) return NERO_ERR_ARG;
@@ -270,9 +257,9 @@ int chain_dispatch(const ChainParams& p, cudaStream_t stream) {
     attr_set = true;
   }
   const int grid = tiles_cap < kNumSMs ? tiles_cap : kNumSMs;
-  if (fam == 0) gemm_chain_kernel<0><<<grid, kChThreads, kChSmemBytes, stream>>>(p);
-  else if (fam == 1) gemm_chain_kernel<1><<<grid, kChThreads, kChSmemBytes, stream>>>(p);
-  else gemm_chain_kernel<2><<<grid, kChThreads, kChSmemBytes, stream>>>(p);
+  if (fam == 0) gemm_chain_kernel<0><<<grid, kChThreads, kChSmemBytes, (cudaStream_t)stream>>>(p);
+  else if (fam == 1) gemm_chain_kernel<1><<<grid, kChThreads, kChSmemBytes, (cudaStream_t)stream>>>(p);
+  else gemm_chain_kernel<2><<<grid, kChThreads, kChSmemBytes, (cudaStream_t)stream>>>(p);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }

@@ -150,7 +150,15 @@ static int dispatch_epi(const LinearParams& p, cudaStream_t stream) {
   return launch_linear<NPAD, EK_DACT_SOFTPLUS>(p, stream);
 }
 
-int linear_dispatch(const LinearParams& p, cudaStream_t stream) {
+extern "C" int nero_linear(const float* A, int lda, int k_valid, const void* wimg, int n_pad, int k_chunks, const float* bias, int n_bias,
+                           float* out, int ldo, int ncol_out, float oscale, int mode, int act, float act_param,
+                           const float* H, int ldh, float hscale, int dact, const float* V, int ldv, float* out2, int ldo2,
+                           const float* addend, int ldadd, int ncol_main, float* tail, int ldt,
+                           const int* m_ptr, int m_cap, void* stream_) {
+  const LinearParams p{A, lda, k_valid, (const uint8_t*)wimg, n_pad, k_chunks, bias, n_bias, out, ldo, ncol_out, oscale, mode, act, act_param,
+                       H, ldh, hscale, dact, V, ldv, out2, ldo2, addend, ldadd, ncol_main, tail, ldt, m_ptr, m_cap};
+  const cudaStream_t stream = (cudaStream_t)stream_;
+  if (!A || !wimg || !out || ncol_out > n_pad) return NERO_ERR_ARG;
   if (p.k_chunks <= 0 || (p.k_valid & 3) || (p.lda & 3) || (reinterpret_cast<uintptr_t>(p.A) & 15)) return NERO_ERR_ARG;
   if (p.mode == EPI_TANGENT && (!p.H || !p.V || !p.out2 || p.dact != ACT_SOFTPLUS100)) return NERO_ERR_ARG;
   if (p.mode == EPI_MUL_DACT && p.dact != ACT_NONE && !p.H) return NERO_ERR_ARG;

@@ -186,7 +186,14 @@ static int launch_wgrad(const WgradParams& p, int P, int n_tiles, cudaStream_t s
 
 // Accumulates partial[P][rows_partial][ld_partial] for output rows [0, n_rows_pad) and columns [0, k_pad)
 // (k_pad multiple of 64), decomposed into 128-row tiles (grid.y) x {256,128,64}-column tiles (separate launches).
-int wgrad_dispatch(WgradParams p, int n_rows_pad, int k_pad, int P, cudaStream_t stream) {
+extern "C" int nero_wgrad(const float* dY, int ldy, int n_valid, const float* X, int ldx, int k_valid,
+                          const float* dY2, int ldy2, const float* X2, int ldx2,
+                          float* partial, int ld_partial, int rows_partial, float* bias_partial,
+                          int n_rows_pad, int k_pad, int P, const int* m_ptr, int m_cap, void* stream_) {
+  WgradParams p{dY, ldy, X, ldx, dY2, ldy2, X2, ldx2, 0, n_valid, 0, k_valid, partial, ld_partial, rows_partial, bias_partial,
+                m_ptr, m_cap};
+  const cudaStream_t stream = (cudaStream_t)stream_;
+  if (!dY || !X || !partial || (dY2 && !X2)) return NERO_ERR_ARG;
   if ((p.ld_partial & 3) || k_pad % 64 || n_rows_pad % 16 || P <= 0) return NERO_ERR_ARG;
   const int n_tiles = (n_rows_pad + 127) / 128;
   p.n0 = 0;

@@ -10,7 +10,6 @@
 #include "math_shade.cuh"
 #include "tile_io.cuh"
 #include "math_mc.cuh"
-#include "../../include/nero_b200.h"
 
 namespace nero {
 
@@ -374,50 +373,61 @@ __global__ void mc_dir_bwd_kernel(const McParams q) {
 
 static inline int blocks_for_l(long n, int per) { return int((n + per - 1) / per); }
 
-int mc_sample(const McParams& q, cudaStream_t st) {
-  const long N = long(q.P) * (q.Sd + q.Ss);
+extern "C" {
+
+int nero_mc_sample(const nero_mc_params* q, void* stream) {
+  if (!q) return NERO_ERR_ARG;
+  const long N = long(q->P) * (q->Sd + q->Ss);
   if (N <= 0) return NERO_OK;
-  mc_sample_kernel<<<blocks_for_l(N, 128), 128, 0, st>>>(q);
+  mc_sample_kernel<<<blocks_for_l(N, 128), 128, 0, (cudaStream_t)stream>>>(*q);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int mc_classify(const McParams& q, cudaStream_t st) {
-  const long N = long(q.P) * (q.Sd + q.Ss);
+int nero_mc_classify(const nero_mc_params* q, void* stream) {
+  if (!q) return NERO_ERR_ARG;
+  const long N = long(q->P) * (q->Sd + q->Ss);
   if (N <= 0) return NERO_OK;
   const int nblk = blocks_for_l(N, kClsBlock);
-  mc_count_kernel<<<nblk, kClsBlock, 0, st>>>(q, N);
+  const cudaStream_t st = (cudaStream_t)stream;
+  mc_count_kernel<<<nblk, kClsBlock, 0, st>>>(*q, N);
   NERO_LAUNCH_CHECK();
-  mc_scan_kernel<<<1, 1024, 0, st>>>(q, nblk, N);
+  mc_scan_kernel<<<1, 1024, 0, st>>>(*q, nblk, N);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int mc_fill(const McParams& q, cudaStream_t st) {
-  const long N = long(q.P) * (q.Sd + q.Ss);
+int nero_mc_fill(const nero_mc_params* q, void* stream) {
+  if (!q) return NERO_ERR_ARG;
+  const long N = long(q->P) * (q->Sd + q->Ss);
   if (N <= 0) return NERO_OK;
   static const cudaError_t attr = cudaFuncSetAttribute(mc_fill_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMcFillSmem);
   if (attr != cudaSuccess) return NERO_ERR_CUDA;
-  mc_fill_kernel<<<blocks_for_l(N, kClsBlock), kClsBlock, kMcFillSmem, st>>>(q, N);
+  mc_fill_kernel<<<blocks_for_l(N, kClsBlock), kClsBlock, kMcFillSmem, (cudaStream_t)stream>>>(*q, N);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int mc_combine_fwd(const McParams& q, cudaStream_t st) {
-  if (q.P <= 0) return NERO_OK;
-  mc_combine_fwd_kernel<<<blocks_for_l(long(q.P) * 32, 128), 128, 0, st>>>(q);
+int nero_mc_combine_fwd(const nero_mc_params* q, void* stream) {
+  if (!q) return NERO_ERR_ARG;
+  if (q->P <= 0) return NERO_OK;
+  mc_combine_fwd_kernel<<<blocks_for_l(long(q->P) * 32, 128), 128, 0, (cudaStream_t)stream>>>(*q);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int mc_combine_bwd(const McParams& q, cudaStream_t st) {
-  if (q.P <= 0) return NERO_OK;
-  mc_combine_bwd_kernel<<<blocks_for_l(long(q.P) * 32, 128), 128, 0, st>>>(q);
+int nero_mc_combine_bwd(const nero_mc_params* q, void* stream) {
+  if (!q) return NERO_ERR_ARG;
+  if (q->P <= 0) return NERO_OK;
+  mc_combine_bwd_kernel<<<blocks_for_l(long(q->P) * 32, 128), 128, 0, (cudaStream_t)stream>>>(*q);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int mc_dir_bwd(const McParams& q, cudaStream_t st) {
-  if (q.P <= 0) return NERO_OK;
-  mc_dir_bwd_kernel<<<blocks_for_l(long(q.P) * 32, 128), 128, 0, st>>>(q);
+int nero_mc_dir_bwd(const nero_mc_params* q, void* stream) {
+  if (!q) return NERO_ERR_ARG;
+  if (q->P <= 0) return NERO_OK;
+  mc_dir_bwd_kernel<<<blocks_for_l(long(q->P) * 32, 128), 128, 0, (cudaStream_t)stream>>>(*q);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
+
+}  // extern "C"
 
 // PE8 rows of the material network input (MaterialFeatsNetwork, field.py:660-689): X [M,ldx] cols 0..50, the same 51
 // columns at CAT[:, 256..306] (skip concat before module1) and the raw xyz at Y[:, 256..258] (predictor input cat(feats, pts)).
@@ -430,9 +440,9 @@ __global__ void mat_prep_kernel(const float* __restrict__ pts, int M, float* X, 
   for (int c = 0; c < 51; ++c) { X[size_t(i) * ldx + c] = pe[c]; CAT[size_t(i) * ldc + 256 + c] = pe[c]; }
   for (int c = 0; c < 3; ++c) Y[size_t(i) * ldy + 256 + c] = p[c];
 }
-int mat_prep(const float* pts, int M, float* X, int ldx, float* CAT, int ldc, float* Y, int ldy, cudaStream_t st) {
+extern "C" int nero_mat_prep(const float* pts, int M, float* X, int ldx, float* CAT, int ldc, float* Y, int ldy, void* stream) {
   if (M <= 0) return NERO_OK;
-  mat_prep_kernel<<<(M + 127) / 128, 128, 0, st>>>(pts, M, X, ldx, CAT, ldc, Y, ldy);
+  mat_prep_kernel<<<(M + 127) / 128, 128, 0, (cudaStream_t)stream>>>(pts, M, X, ldx, CAT, ldc, Y, ldy);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }

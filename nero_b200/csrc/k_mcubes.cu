@@ -235,7 +235,11 @@ bool mcb_grid(const float* u, int nx, int ny, int nz, float iso, McGrid& g, int&
 
 }  // namespace
 
-int mcubes_count(const float* u, int nx, int ny, int nz, float iso, int* blk_cnt, long long* blk_off, long long* totals, cudaStream_t st) {
+extern "C" {
+
+int nero_mcubes_count(const float* u, int nx, int ny, int nz, float iso, int* blk_cnt, long long* blk_off, long long* totals,
+                      void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
   McGrid g;
   int nblk;
   if (!mcb_grid(u, nx, ny, nz, iso, g, nblk) || !blk_cnt || !blk_off || !totals) return NERO_ERR_ARG;
@@ -245,8 +249,9 @@ int mcubes_count(const float* u, int nx, int ny, int nz, float iso, int* blk_cnt
   return NERO_OK;
 }
 
-int mcubes_emit(const float* u, int nx, int ny, int nz, float iso, const long long* blk_off, long long V, long long T, int* emap,
-                float* verts, int* tris, cudaStream_t st) {
+int nero_mcubes_emit(const float* u, int nx, int ny, int nz, float iso, const long long* blk_off, long long V, long long T, int* emap,
+                     float* verts, int* tris, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
   McGrid g;
   int nblk;
   if (!mcb_grid(u, nx, ny, nz, iso, g, nblk) || !blk_off) return NERO_ERR_ARG;
@@ -258,5 +263,7 @@ int mcubes_emit(const float* u, int nx, int ny, int nz, float iso, const long lo
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
+
+}  // extern "C"
 
 }  // namespace nero

@@ -7,7 +7,6 @@
 // Per path: jittered camera ray -> closest hit; at each hit, next-event estimation from the importance-sampled environment
 // with an any-hit shadow ray, and a BRDF sample (diffuse or GGX lobe) that continues the path; the two are combined with
 // the power heuristic.  No Russian roulette: at most 1 + 2 * max_bounces rays per path.
-#include "../../include/nero_b200.h"
 #include "bvh_traverse.cuh"
 #include "common.cuh"
 #include "math_relight.cuh"
@@ -150,13 +149,15 @@ __global__ void __launch_bounds__(128) relight_kernel(const nero_relight_params 
 
 }  // namespace
 
-int relight_render(const nero_relight_params& q, cudaStream_t st) {
+extern "C" int nero_relight_render(const nero_relight_params* p, void* stream) {
+  if (!p) return NERO_ERR_ARG;
+  const nero_relight_params& q = *p;
   if (!q.nodes || !q.tris || !q.tri_ids || !q.faces || !q.vmat || !q.env || !q.env_p || !q.cdf_rows || !q.cdf_cols || !q.accum)
     return NERO_ERR_ARG;
   if (q.env_w < 1 || q.env_h < 1 || q.width < 1 || q.height < 1 || q.spp0 < 0 || q.spp < 0 || q.max_bounces < 1) return NERO_ERR_ARG;
   if (q.spp == 0) return NERO_OK;
   const dim3 grid((q.width + 15) / 16, (q.height + 7) / 8);
-  relight_kernel<<<grid, 128, 0, st>>>(q);
+  relight_kernel<<<grid, 128, 0, (cudaStream_t)stream>>>(q);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }

@@ -466,114 +466,131 @@ __global__ void composite_kernel(const int* __restrict__ slot, int R, int S, con
   }
 }
 
-// ------------------------------------------------------------------ host launchers
+// ------------------------------------------------------------------ C ABI entry points (include/nero_b200.h)
 
-int ray_prepare(const float* rays_o, const float* rays_d, const float* z_vals, int R, int S, int* cnt_in, int* cnt_out,
-                int* off_in, int* off_out, int* n_in, int* n_out, cudaStream_t st) {
+extern "C" {
+
+int nero_ray_prepare(const float* rays_o, const float* rays_d, const float* z_vals, int R, int S, int* cnt_in, int* cnt_out,
+                     int* off_in, int* off_out, int* n_in, int* n_out, void* stream) {
   if (R <= 0) return NERO_OK;
+  const cudaStream_t st = (cudaStream_t)stream;
   ray_classify_kernel<<<blocks_for(long(R) * 32, 256), 256, 0, st>>>(rays_o, rays_d, z_vals, R, S, cnt_in, cnt_out);
   ray_scan_kernel<<<1, 1024, 0, st>>>(cnt_in, cnt_out, R, off_in, off_out, n_in, n_out);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int reg_prepare(const float* rays_o, const float* rays_d, const float* z_vals, int R, int S, float radius, int* cnt, int* cnt_dummy,
-                int* off, int* off_dummy, int* n, int* n_dummy, cudaStream_t st) {
+int nero_reg_prepare(const float* rays_o, const float* rays_d, const float* z_vals, int R, int S, float radius, int* cnt, int* cnt_dummy,
+                     int* off, int* off_dummy, int* n, int* n_dummy, void* stream) {
   if (R <= 0) return NERO_OK;
+  const cudaStream_t st = (cudaStream_t)stream;
   reg_classify_kernel<<<blocks_for(long(R) * 32, 256), 256, 0, st>>>(rays_o, rays_d, z_vals, R, S, radius, cnt);
   ray_scan_kernel<<<1, 1024, 0, st>>>(cnt, cnt_dummy, R, off, off_dummy, n, n_dummy);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int reg_fill(const float* rays_o, const float* rays_d, const float* z_vals, int R, int S, float radius, const int* off, float* pts,
-             float* X0, int ldx, float* H4, int ldh, cudaStream_t st) {
+int nero_reg_fill(const float* rays_o, const float* rays_d, const float* z_vals, int R, int S, float radius, const int* off, float* pts,
+                  float* X0, int ldx, float* H4, int ldh, void* stream) {
   if (R <= 0) return NERO_OK;
-  reg_fill_kernel<<<blocks_for(long(R) * 32, 128), 128, 0, st>>>(rays_o, rays_d, z_vals, R, S, radius, off, pts, X0, ldx, H4, ldh);
+  reg_fill_kernel<<<blocks_for(long(R) * 32, 128), 128, 0, (cudaStream_t)stream>>>(rays_o, rays_d, z_vals, R, S, radius, off, pts, X0, ldx,
+                                                                                   H4, ldh);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int points_fill(const float* pts3, int N, float* pts, int* ray_in, float* X0, int ldx, float* Y8, int ldy, float* H4, int ldh, cudaStream_t st) {
+int nero_points_fill(const float* pts3, int N, float* pts, int* ray_in, float* X0, int ldx, float* Y8, int ldy, float* H4, int ldh, void* stream) {
   if (N <= 0) return NERO_OK;
-  points_fill_kernel<<<blocks_for(N, 128), 128, 0, st>>>(pts3, N, pts, ray_in, X0, ldx, Y8, ldy, H4, ldh);
+  points_fill_kernel<<<blocks_for(N, 128), 128, 0, (cudaStream_t)stream>>>(pts3, N, pts, ray_in, X0, ldx, Y8, ldy, H4, ldh);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int ray_fill(const FillParams& q, cudaStream_t st) {
-  if (q.R <= 0) return NERO_OK;
-  ray_fill_kernel<<<blocks_for(long(q.R) * 32, 128), 128, 0, st>>>(q);
+int nero_ray_fill(const float* rays_o, const float* rays_d, const float* z_vals, int R, int S, const int* off_in, const int* off_out,
+                  int* slot, float* pts, int* ray_in, float* X0, int ld_x0, float* Y8, int ld_y8, float* H4, int ld_h4,
+                  float* XN, int ld_xn, float* H5, int ld_h5, float* FV, int ld_fv, float* dist_out, int* ray_out, void* stream) {
+  if (R <= 0) return NERO_OK;
+  const FillParams q{rays_o, rays_d, z_vals, R, S, off_in, off_out, slot, pts, ray_in, X0, ld_x0, Y8, ld_y8, H4, ld_h4, XN, ld_xn, H5, ld_h5,
+                     FV, ld_fv, dist_out, ray_out};
+  ray_fill_kernel<<<blocks_for(long(R) * 32, 128), 128, 0, (cudaStream_t)stream>>>(q);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int dact_times_row(const float* H, int ldh, const float* row, float* V, int ldv, int ncol, const int* m_ptr, int m_cap, cudaStream_t st) {
+int nero_dact_times_row(const float* H, int ldh, const float* row, float* V, int ldv, int ncol, const int* m_ptr, int m_cap, void* stream) {
   if (m_cap <= 0) return NERO_OK;
-  dact_times_row_kernel<<<kNumSMs * 8, 256, 0, st>>>(H, ldh, row, V, ldv, ncol, m_ptr, m_cap);
+  dact_times_row_kernel<<<kNumSMs * 8, 256, 0, (cudaStream_t)stream>>>(H, ldh, row, V, ldv, ncol, m_ptr, m_cap);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int row_axpy(const float* a, int lda, const float* X, int ldx, float* Y, int ldy, int ncol, const int* m_ptr, int m_cap, cudaStream_t st) {
+int nero_row_axpy(const float* a, int lda, const float* X, int ldx, float* Y, int ldy, int ncol, const int* m_ptr, int m_cap, void* stream) {
   if (m_cap <= 0) return NERO_OK;
   if ((ncol & 3) || (ldx & 3) || (ldy & 3)) return NERO_ERR_ARG;
-  row_axpy_kernel<<<kNumSMs * 8, 256, 0, st>>>(a, lda, X, ldx, Y, ldy, ncol, m_ptr, m_cap);
+  row_axpy_kernel<<<kNumSMs * 8, 256, 0, (cudaStream_t)stream>>>(a, lda, X, ldx, Y, ldy, ncol, m_ptr, m_cap);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int pe_grad(const float* X0, int ldx, const float* U0, int ldu, const float* US, int lds, float* G, const int* m_ptr, int m_cap, cudaStream_t st) {
+int nero_pe_grad(const float* X0, int ldx, const float* U0, int ldu, const float* US, int lds, float* G, const int* m_ptr, int m_cap, void* stream) {
   if (m_cap <= 0) return NERO_OK;
-  pe_grad_kernel<<<blocks_for(m_cap, 128), 128, 0, st>>>(X0, ldx, U0, ldu, US, lds, G, m_ptr, m_cap);
+  pe_grad_kernel<<<blocks_for(m_cap, 128), 128, 0, (cudaStream_t)stream>>>(X0, ldx, U0, ldu, US, lds, G, m_ptr, m_cap);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int pe_tangent_launch(const float* X0, int ldx, const float* DG, float* UB0, int ld0, float* UB4, int ld4, const int* m_ptr, int m_cap, cudaStream_t st) {
+int nero_pe_tangent(const float* X0, int ldx, const float* DG, float* UB0, int ld0, float* UB4, int ld4, const int* m_ptr, int m_cap, void* stream) {
   if (m_cap <= 0) return NERO_OK;
-  pe_tangent_kernel<<<blocks_for(m_cap, 128), 128, 0, st>>>(X0, ldx, DG, UB0, ld0, UB4, ld4, m_ptr, m_cap);
+  pe_tangent_kernel<<<blocks_for(m_cap, 128), 128, 0, (cudaStream_t)stream>>>(X0, ldx, DG, UB0, ld0, UB4, ld4, m_ptr, m_cap);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int sdf_alpha_forward(const float* Y8, int ldy, int sdf_col, const float* G, const float* pts, const int* ray_in, const float* rays_d,
-                      const float* variance, const float* car, float* alpha, float* gerr, const int* m_ptr, int m_cap, cudaStream_t st) {
+int nero_sdf_alpha_fwd(const float* Y8, int ldy, int sdf_col, const float* G, const float* pts, const int* ray_in, const float* rays_d,
+                       const float* variance, const float* car, float* alpha, float* gerr, const int* m_ptr, int m_cap, void* stream) {
   if (m_cap <= 0) return NERO_OK;
-  sdf_alpha_fwd_kernel<<<blocks_for(m_cap, 256), 256, 0, st>>>(Y8, ldy, sdf_col, G, pts, ray_in, rays_d, variance, car, alpha, gerr, m_ptr, m_cap);
+  sdf_alpha_fwd_kernel<<<blocks_for(m_cap, 256), 256, 0, (cudaStream_t)stream>>>(Y8, ldy, sdf_col, G, pts, ray_in, rays_d, variance, car, alpha,
+                                                                                 gerr, m_ptr, m_cap);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int sdf_alpha_backward(const float* Y8, int ldy, int sdf_col, const float* G, const float* pts, const int* ray_in, const float* rays_d,
+int nero_sdf_alpha_bwd(const float* Y8, int ldy, int sdf_col, const float* G, const float* pts, const int* ray_in, const float* rays_d,
                        const float* variance, const float* car, const float* dalpha, const float* dgerr, float* dY8, int lddy, float* DG,
-                       float* d_inv_s, const int* m_ptr, int m_cap, cudaStream_t st) {
+                       float* d_inv_s, const int* m_ptr, int m_cap, void* stream) {
   if (m_cap <= 0) return NERO_OK;
   const int nb = blocks_for(m_cap, 256);
   if (nb > kDinvsMaxBlocks) return NERO_ERR_ARG;
+  const cudaStream_t st = (cudaStream_t)stream;
   sdf_alpha_bwd_kernel<<<nb, 256, 0, st>>>(Y8, ldy, sdf_col, G, pts, ray_in, rays_d, variance, car, dalpha, dgerr, dY8, lddy, DG, d_inv_s, m_ptr, m_cap);
   sdf_alpha_bwd_finish_kernel<<<1, 256, 0, st>>>(nb, d_inv_s);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int nerf_post_forward(const float* dens, int ldd, const float* rgb, int ldr, const float* dist, float* alpha, float* color, const int* m_ptr, int m_cap, cudaStream_t st) {
+int nero_nerf_post_fwd(const float* dens, int ldd, const float* rgb, int ldr, const float* dist, float* alpha, float* color,
+                       const int* m_ptr, int m_cap, void* stream) {
   if (m_cap <= 0) return NERO_OK;
-  nerf_post_fwd_kernel<<<blocks_for(m_cap, 256), 256, 0, st>>>(dens, ldd, rgb, ldr, dist, alpha, color, m_ptr, m_cap);
+  nerf_post_fwd_kernel<<<blocks_for(m_cap, 256), 256, 0, (cudaStream_t)stream>>>(dens, ldd, rgb, ldr, dist, alpha, color, m_ptr, m_cap);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int nerf_post_backward(const float* dens, int ldd, const float* rgb, int ldr, const float* dist, const float* dalpha, const float* dcolor,
-                       float* ddens, int lddd, float* drgb, int lddr, const int* m_ptr, int m_cap, cudaStream_t st) {
+int nero_nerf_post_bwd(const float* dens, int ldd, const float* rgb, int ldr, const float* dist, const float* dalpha, const float* dcolor,
+                       float* ddens, int lddd, float* drgb, int lddr, const int* m_ptr, int m_cap, void* stream) {
   if (m_cap <= 0) return NERO_OK;
-  nerf_post_bwd_kernel<<<blocks_for(m_cap, 256), 256, 0, st>>>(dens, ldd, rgb, ldr, dist, dalpha, dcolor, ddens, lddd, drgb, lddr, m_ptr, m_cap);
+  nerf_post_bwd_kernel<<<blocks_for(m_cap, 256), 256, 0, (cudaStream_t)stream>>>(dens, ldd, rgb, ldr, dist, dalpha, dcolor, ddens, lddd, drgb,
+                                                                                 lddr, m_ptr, m_cap);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int composite_forward(const int* slot, int R, int S, const float* a_in, const float* c_in, const float* a_out, const float* c_out,
-                      float* rgb, float* weights, cudaStream_t st) {
+int nero_composite_fwd(const int* slot, int R, int S, const float* a_in, const float* c_in, const float* a_out, const float* c_out,
+                       float* rgb, float* weights, void* stream) {
   if (R <= 0) return NERO_OK;
   if (S > 256) return NERO_ERR_ARG;
-  composite_kernel<false><<<blocks_for(long(R) * 32, 128), 128, 0, st>>>(slot, R, S, a_in, c_in, a_out, c_out, rgb, weights, nullptr, nullptr, nullptr, nullptr, nullptr);
+  composite_kernel<false><<<blocks_for(long(R) * 32, 128), 128, 0, (cudaStream_t)stream>>>(slot, R, S, a_in, c_in, a_out, c_out, rgb, weights,
+                                                                                           nullptr, nullptr, nullptr, nullptr, nullptr);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int composite_backward(const int* slot, int R, int S, const float* a_in, const float* c_in, const float* a_out, const float* c_out,
-                       const float* drgb, float* da_in, float* dc_in, float* da_out, float* dc_out, cudaStream_t st) {
+int nero_composite_bwd(const int* slot, int R, int S, const float* a_in, const float* c_in, const float* a_out, const float* c_out,
+                       const float* drgb, float* da_in, float* dc_in, float* da_out, float* dc_out, void* stream) {
   if (R <= 0) return NERO_OK;
   if (S > 256) return NERO_ERR_ARG;
-  composite_kernel<true><<<blocks_for(long(R) * 32, 128), 128, 0, st>>>(slot, R, S, a_in, c_in, a_out, c_out, nullptr, nullptr, drgb, da_in, dc_in, da_out, dc_out);
+  composite_kernel<true><<<blocks_for(long(R) * 32, 128), 128, 0, (cudaStream_t)stream>>>(slot, R, S, a_in, c_in, a_out, c_out, nullptr, nullptr,
+                                                                                          drgb, da_in, dc_in, da_out, dc_out);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
+
+}  // extern "C"
 
 }  // namespace nero

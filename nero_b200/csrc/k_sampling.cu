@@ -314,51 +314,66 @@ __global__ void occ_loss_kernel(const float* __restrict__ occ_prob, const float*
 
 static inline int blocks_for(long n, int per) { return int((n + per - 1) / per); }
 
-int sample_init(const SampleInitParams& q, cudaStream_t st) {
-  if (q.R <= 0) return NERO_OK;
-  if (q.nb > q.n) return NERO_ERR_ARG;
-  sample_init_kernel<<<blocks_for(long(q.R) * q.n, 128), 128, 0, st>>>(q);
+extern "C" {
+
+int nero_sample_init(const float* rays_o, const float* rays_d, const float* near, const float* far, int R, int n, int nb,
+                     const float* lin_inner, const float* bg_base, const float* bg_lower, const float* bg_upper,
+                     const float* rand_inner, const float* rand_bg, float* z, int ldz, float* z_bg, int ldzb,
+                     float* X0, int ldx, float* HC, int ldh, void* stream) {
+  if (R <= 0) return NERO_OK;
+  if (nb > n) return NERO_ERR_ARG;
+  const SampleInitParams q{rays_o, rays_d, near, far, R, n, nb, lin_inner, bg_base, bg_lower, bg_upper, rand_inner, rand_bg, z, ldz, z_bg,
+                           ldzb, X0, ldx, HC, ldh};
+  sample_init_kernel<<<blocks_for(long(R) * n, 128), 128, 0, (cudaStream_t)stream>>>(q);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int upsample(const UpsampleParams& q, cudaStream_t st) {
-  if (q.R <= 0) return NERO_OK;
-  if (q.n > kMaxN || q.n_new > 32 || q.n < 2) return NERO_ERR_ARG;
-  upsample_kernel<<<blocks_for(q.R, 4), 128, 0, st>>>(q);
+int nero_upsample(const float* rays_o, const float* rays_d, int R, const float* z, int ldz, const float* sdf, int lds, int n, int n_new,
+                  const float* variance, float inv_s_cap, int clip, int surface_variant, float* new_z, int ldn,
+                  float* X0, int ldx, float* HC, int ldh, float* wsum, void* stream) {
+  if (R <= 0) return NERO_OK;
+  if (n > kMaxN || n_new > 32 || n < 2) return NERO_ERR_ARG;
+  const UpsampleParams q{rays_o, rays_d, R, z, ldz, sdf, lds, n, n_new, variance, inv_s_cap, clip, surface_variant, new_z, ldn, X0, ldx, HC,
+                         ldh, wsum, nullptr};
+  upsample_kernel<<<blocks_for(R, 4), 128, 0, (cudaStream_t)stream>>>(q);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int merge_samples(const float* z, int ldz, const float* sdf, int lds, int n, const float* nz, int ldn, const float* nsdf, int ldns,
-                  int m, float* oz, int ldoz, float* osdf, int ldos, int R, cudaStream_t st) {
+int nero_merge_samples(const float* z, int ldz, const float* sdf, int lds, int n, const float* nz, int ldn, const float* nsdf, int ldns,
+                       int m, float* oz, int ldoz, float* osdf, int ldos, int R, void* stream) {
   if (R <= 0) return NERO_OK;
   if (n > kMaxN || m > 32) return NERO_ERR_ARG;
-  merge_kernel<<<blocks_for(R, 4), 128, 0, st>>>(z, ldz, sdf, lds, n, nz, ldn, nsdf, ldns, m, oz, ldoz, osdf, ldos, R);
+  merge_kernel<<<blocks_for(R, 4), 128, 0, (cudaStream_t)stream>>>(z, ldz, sdf, lds, n, nz, ldn, nsdf, ldns, m, oz, ldoz, osdf, ldos, R);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int occ_init(const float* pts, const float* refl, const int* sel, const int* p_ptr, int p_cap, int sn0, const float* lin,
-             float* o_out, float* d_out, float* z, int ldz, float* X0, int ldx, float* HC, int ldh, cudaStream_t st) {
+int nero_occ_init(const float* pts, const float* refl, const int* sel, const int* p_ptr, int p_cap, int sn0, const float* lin,
+                  float* o_out, float* d_out, float* z, int ldz, float* X0, int ldx, float* HC, int ldh, void* stream) {
   if (p_cap <= 0) return NERO_OK;
-  occ_init_kernel<<<blocks_for(long(p_cap) * sn0, 128), 128, 0, st>>>(pts, refl, sel, p_ptr, p_cap, sn0, lin, o_out, d_out, z, ldz, X0, ldx, HC, ldh);
+  occ_init_kernel<<<blocks_for(long(p_cap) * sn0, 128), 128, 0, (cudaStream_t)stream>>>(pts, refl, sel, p_ptr, p_cap, sn0, lin, o_out, d_out, z,
+                                                                                        ldz, X0, ldx, HC, ldh);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int occ_select(const float* pts, const float* Y8, int ldy, int sdf_col, const float* G, const int* ray_in, const float* rays_d,
-               float sdf_thresh, const int* m_ptr, int m_cap, int* sel, int* count, cudaStream_t st) {
+int nero_occ_select(const float* pts, const float* Y8, int ldy, int sdf_col, const float* G, const int* ray_in, const float* rays_d,
+                    float sdf_thresh, const int* m_ptr, int m_cap, int* sel, int* count, void* stream) {
   if (m_cap <= 0) return NERO_OK;
   const int nb = blocks_for(m_cap, 1024);
   if (nb > kOccMaxBlocks) return NERO_ERR_ARG;
+  const cudaStream_t st = (cudaStream_t)stream;
   occ_select_kernel<0><<<nb, 1024, 0, st>>>(pts, Y8, ldy, sdf_col, G, ray_in, rays_d, sdf_thresh, m_ptr, m_cap, sel, count);
   occ_select_kernel<1><<<nb, 1024, 0, st>>>(pts, Y8, ldy, sdf_col, G, ray_in, rays_d, sdf_thresh, m_ptr, m_cap, sel, count);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int occ_loss(const float* occ_prob, const float* gt, const int* sel, const int* p_ptr, int p_cap, float* loss_sum, float* docc_sign,
-             cudaStream_t st) {
+int nero_occ_loss(const float* occ_prob, const float* gt, const int* sel, const int* p_ptr, int p_cap, float* loss_sum, float* docc_sign,
+                  void* stream) {
   if (p_cap <= 0) return NERO_OK;
-  occ_loss_kernel<<<1, kOccLossThreads, 0, st>>>(occ_prob, gt, sel, p_ptr, p_cap, loss_sum, docc_sign);
+  occ_loss_kernel<<<1, kOccLossThreads, 0, (cudaStream_t)stream>>>(occ_prob, gt, sel, p_ptr, p_cap, loss_sum, docc_sign);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
+
+}  // extern "C"
 
 }  // namespace nero

@@ -258,40 +258,53 @@ __global__ void __launch_bounds__(kEncBlock) ide_kernel(const float* __restrict_
   }
 }
 
-int ide_standalone(const float* dirs, int ldd, const float* kappa, int kstride, float kappa_scalar, int M, float* out, int ldo, cudaStream_t st) {
-  if (!dirs || !out || ldd < 3 || ldo < 72) return NERO_ERR_ARG;
-  if (M <= 0) return NERO_OK;
-  ide_kernel<<<(M + kEncBlock - 1) / kEncBlock, kEncBlock, 0, st>>>(dirs, ldd, kappa, kstride, kappa_scalar, M, out, ldo);
-  NERO_LAUNCH_CHECK();
-  return NERO_OK;
-}
-
-
 static inline int blocks_for(long n, int per) { return int((n + per - 1) / per); }
 
-int shade_prep_forward(const ShadePrepParams& q, cudaStream_t st) {
-  if (q.m_cap <= 0) return NERO_OK;
-  shade_prep_fwd_kernel<<<blocks_for(q.m_cap, 128), 128, 0, st>>>(q);
+extern "C" {
+
+int nero_ide(const float* dirs, int ldd, const float* kappa_inv, int kstride, float kappa_scalar, int M, float* out, int ldo, void* stream) {
+  if (!dirs || !out || ldd < 3 || ldo < 72) return NERO_ERR_ARG;
+  if (M <= 0) return NERO_OK;
+  ide_kernel<<<(M + kEncBlock - 1) / kEncBlock, kEncBlock, 0, (cudaStream_t)stream>>>(dirs, ldd, kappa_inv, kstride, kappa_scalar, M, out, ldo);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int shade_prep_backward(const ShadePrepBwdParams& q, cudaStream_t st) {
-  if (q.m_cap <= 0) return NERO_OK;
-  shade_prep_bwd_kernel<<<blocks_for(q.m_cap, 128), 128, 0, st>>>(q);
+int nero_shade_prep_fwd(const float* G, const float* pts, const int* ray_in, const float* rays_d, const float* OUTS, float* E, int lde,
+                        float* GEO, const float* human_poses, float* EH, int ldeh, int pos_freq, const int* m_ptr, int m_cap, int sphere, void* stream) {
+  if (m_cap <= 0) return NERO_OK;
+  const ShadePrepParams q{G, pts, ray_in, rays_d, OUTS, E, lde, GEO, human_poses, EH, ldeh, pos_freq, m_ptr, m_cap, sphere};
+  shade_prep_fwd_kernel<<<blocks_for(m_cap, 128), 128, 0, (cudaStream_t)stream>>>(q);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int shade_combine_forward(const ShadeCombineParams& q, cudaStream_t st) {
-  if (q.m_cap <= 0) return NERO_OK;
-  shade_combine_fwd_kernel<<<blocks_for(q.m_cap, 256), 256, 0, st>>>(q);
+int nero_shade_prep_bwd(const float* G, const float* pts, const int* ray_in, const float* rays_d, const float* OUTS, const float* GEO,
+                        const float* dE_dir, int ld_dir, const float* dE_inn, int ld_inn, const float* dE_dif, int ld_dif,
+                        const float* dEH, int ld_eh, const float* human_poses, const float* dNoV, float* DOUTS, float* DG,
+                        const int* m_ptr, int m_cap, int sphere, void* stream) {
+  if (m_cap <= 0) return NERO_OK;
+  const ShadePrepBwdParams q{G, pts, ray_in, rays_d, OUTS, GEO, dE_dir, ld_dir, dE_inn, ld_inn, dE_dif, ld_dif, dEH, ld_eh, human_poses, dNoV,
+                             DOUTS, DG, m_ptr, m_cap, sphere};
+  shade_prep_bwd_kernel<<<blocks_for(m_cap, 128), 128, 0, (cudaStream_t)stream>>>(q);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
-int shade_combine_backward(const ShadeCombineParams& q, cudaStream_t st) {
-  if (q.m_cap <= 0) return NERO_OK;
-  shade_combine_bwd_kernel<<<blocks_for(q.m_cap, 256), 256, 0, st>>>(q);
+int nero_shade_combine_fwd(const float* OUTS, const float* GEO, const float* lut, float exp_max, int human, float* color,
+                           float* occ_prob, float* refl, const int* m_ptr, int m_cap, void* stream) {
+  if (m_cap <= 0) return NERO_OK;
+  const ShadeCombineParams q{OUTS, GEO, lut, exp_max, human, color, occ_prob, refl, nullptr, nullptr, nullptr, nullptr, m_ptr, m_cap};
+  shade_combine_fwd_kernel<<<blocks_for(m_cap, 256), 256, 0, (cudaStream_t)stream>>>(q);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
+int nero_shade_combine_bwd(const float* OUTS, const float* GEO, const float* lut, float exp_max, int human, const float* dcolor,
+                           const float* docc, float* DOUTS, float* dNoV, const int* m_ptr, int m_cap, void* stream) {
+  if (m_cap <= 0) return NERO_OK;
+  const ShadeCombineParams q{OUTS, GEO, lut, exp_max, human, nullptr, nullptr, nullptr, dcolor, docc, DOUTS, dNoV, m_ptr, m_cap};
+  shade_combine_bwd_kernel<<<blocks_for(m_cap, 256), 256, 0, (cudaStream_t)stream>>>(q);
+  NERO_LAUNCH_CHECK();
+  return NERO_OK;
+}
+
+}  // extern "C"
 
 }  // namespace nero

@@ -66,32 +66,26 @@ __global__ void prep_weight_kernel(const float* __restrict__ v, const float* __r
   prep_weight_row(blockIdx.x, v, g, K, row0, kmap, in_scale, img_f, rows_pad_f, img_t, rows_pad_t, t_c0, t_ncols, w_eff, ld_weff);
 }
 // all layers of a network in one launch: blockIdx.y selects the job
-struct PrepJob {
-  const float* v; const float* g; const int* kmap; uint8_t* img_f; uint8_t* img_t; float* w_eff;
-  int K, row0, nrows, rows_pad_f, rows_pad_t, t_c0, t_ncols, ld_weff;
-  float in_scale; int pad_;
-};
-static_assert(sizeof(PrepJob) == 88, "PrepJob layout is part of the C ABI (nero_prep_weight_batch)");
-__global__ void prep_weight_batch_kernel(const PrepJob* __restrict__ jobs) {
-  const PrepJob j = jobs[blockIdx.y];
+__global__ void prep_weight_batch_kernel(const nero_prep_job* __restrict__ jobs) {
+  const nero_prep_job j = jobs[blockIdx.y];
   if (int(blockIdx.x) >= j.nrows) return;
-  prep_weight_row(blockIdx.x, j.v, j.g, j.K, j.row0, j.kmap, j.in_scale, j.img_f, j.rows_pad_f, j.img_t, j.rows_pad_t, j.t_c0, j.t_ncols,
-                  j.w_eff, j.ld_weff);
+  prep_weight_row(blockIdx.x, j.v, j.g, j.K, j.row0, j.kmap, j.in_scale, static_cast<uint8_t*>(j.img_f), j.rows_pad_f,
+                  static_cast<uint8_t*>(j.img_t), j.rows_pad_t, j.t_c0, j.t_ncols, j.w_eff, j.ld_weff);
 }
-int prep_weight_batch(const void* jobs_dev, int n_jobs, int max_rows, cudaStream_t stream) {
+extern "C" int nero_prep_weight_batch(const void* jobs_dev, int n_jobs, int max_rows, void* stream) {
   if (n_jobs <= 0 || max_rows <= 0) return NERO_OK;
   if (!jobs_dev) return NERO_ERR_ARG;
-  prep_weight_batch_kernel<<<dim3(max_rows, n_jobs), 128, 0, stream>>>(static_cast<const PrepJob*>(jobs_dev));
+  prep_weight_batch_kernel<<<dim3(max_rows, n_jobs), 128, 0, (cudaStream_t)stream>>>(static_cast<const nero_prep_job*>(jobs_dev));
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
 
-int prep_weight(const float* v, const float* g, int K, int row0, int nrows, const int* kmap, float in_scale,
-                uint8_t* img_f, int rows_pad_f, uint8_t* img_t, int rows_pad_t, int t_c0, int t_ncols, float* w_eff,
-                int ld_weff, cudaStream_t stream) {
+extern "C" int nero_prep_weight(const float* v, const float* g, int K, int row0, int nrows, const int* kmap, float in_scale,
+                                void* img_f, int rows_pad_f, void* img_t, int rows_pad_t, int t_c0, int t_ncols, float* w_eff,
+                                int ld_weff, void* stream) {
   if (nrows <= 0) return NERO_OK;
-  prep_weight_kernel<<<nrows, 128, 0, stream>>>(v, g, K, row0, kmap, in_scale, img_f, rows_pad_f, img_t, rows_pad_t,
-                                                t_c0, t_ncols, w_eff, ld_weff);
+  prep_weight_kernel<<<nrows, 128, 0, (cudaStream_t)stream>>>(v, g, K, row0, kmap, in_scale, static_cast<uint8_t*>(img_f), rows_pad_f,
+                                                              static_cast<uint8_t*>(img_t), rows_pad_t, t_c0, t_ncols, w_eff, ld_weff);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
@@ -162,37 +156,31 @@ __global__ void wgrad_finish_kernel(const float* __restrict__ partial, int P, in
                    extra_row, extra_scale);
 }
 // many layers in one launch: blockIdx.y selects the job (jobs must not share destination rows)
-struct FinishJob {
-  const float* partial; const float* bias_partial; const int* kmap; const float* v; const float* g;
-  float* grad_w; float* grad_g; float* grad_b; const float* extra_row;
-  int P, rows_partial, ld_partial, K, row0, nrows;
-  float in_scale, extra_scale;
-};
-static_assert(sizeof(FinishJob) == 104, "FinishJob layout is part of the C ABI (nero_wgrad_finish_batch)");
-__global__ void wgrad_finish_batch_kernel(const FinishJob* __restrict__ jobs) {
-  const FinishJob j = jobs[blockIdx.y];
+__global__ void wgrad_finish_batch_kernel(const nero_finish_job* __restrict__ jobs) {
+  const nero_finish_job j = jobs[blockIdx.y];
   if (int(blockIdx.x) >= j.nrows) return;
   wgrad_finish_row(blockIdx.x, j.partial, j.P, j.rows_partial, j.ld_partial, j.bias_partial, j.K, j.row0, j.kmap, j.in_scale, j.v, j.g,
                    j.grad_w, j.grad_g, j.grad_b, j.extra_row, j.extra_scale);
 }
-int wgrad_finish_batch(const void* jobs_dev, int n_jobs, int max_rows, int max_k, cudaStream_t stream) {
+extern "C" int nero_wgrad_finish_batch(const void* jobs_dev, int n_jobs, int max_rows, int max_k, void* stream) {
   if (n_jobs <= 0 || max_rows <= 0) return NERO_OK;
   if (!jobs_dev || max_k <= 0 || max_k > 1024) return NERO_ERR_ARG;
   // (256, 4) blocks: four groups of partial slices are summed in parallel (the per-row reads are latency bound)
-  wgrad_finish_batch_kernel<<<dim3(max_rows, n_jobs), dim3(256, 4), 4 * max_k * sizeof(float), stream>>>(static_cast<const FinishJob*>(jobs_dev));
+  wgrad_finish_batch_kernel<<<dim3(max_rows, n_jobs), dim3(256, 4), 4 * max_k * sizeof(float), (cudaStream_t)stream>>>(
+      static_cast<const nero_finish_job*>(jobs_dev));
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
 
-int wgrad_finish(const float* partial, int P, int rows_partial, int ld_partial, const float* bias_partial, int K,
-                 int row0, int nrows, const int* kmap, float in_scale, const float* v, const float* g, float* grad_w,
-                 float* grad_g, float* grad_b, const float* extra_row, float extra_scale, cudaStream_t stream) {
+extern "C" int nero_wgrad_finish(const float* partial, int P, int rows_partial, int ld_partial, const float* bias_partial, int K,
+                                 int row0, int nrows, const int* kmap, float in_scale, const float* v, const float* g, float* grad_w,
+                                 float* grad_g, float* grad_b, const float* extra_row, float extra_scale, void* stream) {
   if (nrows <= 0) return NERO_OK;
   int bx = 32;
   while (bx < K && bx < 256) bx <<= 1;
-  wgrad_finish_kernel<<<nrows, dim3(bx, 4), 4 * K * sizeof(float), stream>>>(partial, P, rows_partial, ld_partial, bias_partial, K, row0,
-                                                                            kmap, in_scale, v, g, grad_w, grad_g, grad_b, extra_row,
-                                                                            extra_scale);
+  wgrad_finish_kernel<<<nrows, dim3(bx, 4), 4 * K * sizeof(float), (cudaStream_t)stream>>>(partial, P, rows_partial, ld_partial, bias_partial,
+                                                                                          K, row0, kmap, in_scale, v, g, grad_w, grad_g,
+                                                                                          grad_b, extra_row, extra_scale);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
@@ -259,13 +247,14 @@ __global__ void colsum_finish_kernel(int ncol, int nparts, float* out) {
   out[col] += t;
 }
 
-int colsum(const float* X, int ldx, int ncol, const float* w, int ldw, const int* m_ptr, int m_cap, float* out,
-           cudaStream_t stream) {
+extern "C" int nero_colsum(const float* X, int ldx, int ncol, const float* w, int ldw, const int* m_ptr, int m_cap, float* out,
+                           void* stream) {
   if (m_cap <= 0 || ncol <= 0) return NERO_OK;
   if (ncol > kColsumMaxCols) return NERO_ERR_ARG;
+  const cudaStream_t st = (cudaStream_t)stream;
   dim3 grid((ncol + 127) / 128, kNumSMs);
-  colsum_kernel<<<grid, 256, 0, stream>>>(X, ldx, ncol, w, ldw, m_ptr, m_cap);
-  colsum_finish_kernel<<<(ncol + 127) / 128, 128, 0, stream>>>(ncol, kNumSMs, out);
+  colsum_kernel<<<grid, 256, 0, st>>>(X, ldx, ncol, w, ldw, m_ptr, m_cap);
+  colsum_finish_kernel<<<(ncol + 127) / 128, 128, 0, st>>>(ncol, kNumSMs, out);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
@@ -301,13 +290,15 @@ __global__ void adam_flat_kernel(float* __restrict__ p, const float* __restrict_
     }
   }
 }
-int adam_flat(float* p, const float* g, float* m, float* v, long n, float lr_over_bc1, float b1, float b2, float eps, float inv_sqrt_bc2,
-              float wd, cudaStream_t st) {
+extern "C" int nero_adam_flat(float* p, const float* g, float* m, float* v, long long n, float lr_over_bc1, float b1, float b2, float eps,
+                              float inv_sqrt_bc2, float weight_decay, void* stream) {
+  if (!p || !g || !m || !v) return NERO_ERR_ARG;
   if (n <= 0) return NERO_OK;
   if ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) | reinterpret_cast<uintptr_t>(v)) & 15)
     return NERO_ERR_ARG;
   const long n4 = (n + 3) / 4;
-  adam_flat_kernel<<<int((n4 + 255) / 256), 256, 0, st>>>(p, g, m, v, n, lr_over_bc1, b1, b2, eps, inv_sqrt_bc2, wd);
+  adam_flat_kernel<<<int((n4 + 255) / 256), 256, 0, (cudaStream_t)stream>>>(p, g, m, v, long(n), lr_over_bc1, b1, b2, eps, inv_sqrt_bc2,
+                                                                            weight_decay);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }

@@ -61,8 +61,7 @@ def upload_ide_table():
     global _ide_uploaded
     if not _ide_uploaded:
         mat = ide_coefficient_table()
-        rc = ops.lib.nero_set_ide_table(mat.ctypes.data_as(ops.ctypes.c_void_p))
-        ops._check(rc, 'nero_set_ide_table')
+        ops.call('nero_set_ide_table', mat)
         _ide_uploaded = True
 
 

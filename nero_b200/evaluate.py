@@ -32,7 +32,6 @@ Three consequences of the reference's rasteriser call, reproduced on purpose:
 Two boundaries are restated rather than pinned (DESIGN.md section 2): nvdiffrast's coverage rule on silhouette edges (a ray
 cast counts a pixel centre on an edge as covered) and Open3D's output order (hash order; here ascending voxel key).
 """
-import ctypes
 import os
 import pickle
 
@@ -57,13 +56,6 @@ def _ops():
 
 
 # ------------------------------------------------------------------------------------------------ depth maps
-class DepthParams(ctypes.Structure):
-    """Mirror of nero_depth_params (include/nero_b200.h)."""
-    _vp, _ci, _cf = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
-    _fields_ = [('nodes', _vp), ('tris', _vp), ('tri_ids', _vp), ('faces', _vp), ('verts', _vp), ('depth', _vp),
-                ('pose', _cf * 12), ('K', _cf * 9), ('width', _ci), ('height', _ci), ('near_z', _cf), ('far_z', _cf)]
-
-
 class DepthRenderer:
     """A triangle mesh resident on the GPU (BVH built once) whose depth maps render() produces as the reference's
     rasterize_depth_map does (rules 1-3 of the module docstring)."""
@@ -92,14 +84,12 @@ class DepthRenderer:
             raise ValueError(f'render_depth needs pinhole intrinsics without skew, got {K.tolist()}')
         if out is None:
             out = torch.empty(h, w, dtype=torch.float32, device=self.dev)
-        q = DepthParams()
-        for name, t in (('nodes', self.nodes), ('tris', self.tri), ('tri_ids', self.tri_ids), ('faces', self.faces),
-                        ('verts', self.verts_d), ('depth', out)):
-            setattr(q, name, t.data_ptr())
+        ops = _ops()
+        q = ops.DepthParams().set(nodes=self.nodes, tris=self.tri, tri_ids=self.tri_ids, faces=self.faces, verts=self.verts_d, depth=out)
         q.pose[:] = [float(x) for x in np.asarray(pose, np.float32).reshape(12)]
         q.K[:] = [float(x) for x in K.astype(np.float32).reshape(9)]
         q.width, q.height, q.near_z, q.far_z = w, h, near, far
-        _ops().mc('nero_depth_render', q)
+        ops.K('nero_depth_render', q)
         return out.view(h, w)
 
 
@@ -142,14 +132,10 @@ def depth_to_points_cuda(depth, poses, Ks, lo=0.0, hi=float('inf')):
     blk_cnt = torch.empty(nblk, dtype=torch.int32, device=d.device)
     blk_off = torch.empty(nblk, dtype=torch.int64, device=d.device)
     total = torch.empty(1, dtype=torch.int64, device=d.device)
-    flo, fhi = ctypes.c_float(lo), ctypes.c_float(hi)
-    ops._check(ops.lib.nero_depth_points_count(ops._ptr(d), nv, h, w, flo, fhi, ops._ptr(blk_cnt), ops._ptr(blk_off), ops._ptr(total),
-                                               ops._stream()), 'nero_depth_points_count')
+    ops.K('nero_depth_points_count', d, nv, h, w, lo, hi, blk_cnt, blk_off, total, launches=2)
     n = int(total.item())
     pts = torch.empty(n, 3, dtype=torch.float32, device=d.device)
-    ops._check(ops.lib.nero_depth_points_emit(ops._ptr(d), nv, h, w, flo, fhi, ops._ptr(cams), ops._ptr(blk_off), ctypes.c_longlong(n),
-                                              ops._ptr(pts), ops._stream()), 'nero_depth_points_emit')
-    ops.launch_count += 2 + (n > 0)
+    ops.K('nero_depth_points_emit', d, nv, h, w, lo, hi, cams, blk_off, n, pts, launches=int(n > 0))
     return pts
 
 
@@ -184,16 +170,13 @@ def voxel_down_sample_cuda(pts, voxel=VOXEL):
     if (np.floor((bounds[3:] - bounds[:3]) / voxel) >= _KEY_LIMIT).any() or not np.isfinite(bounds).all():
         raise ValueError(f'voxel_down_sample: extent {hi - lo} at voxel {voxel} needs more than {_KEY_LIMIT} cells along an axis')
     keys = torch.empty(n, dtype=torch.int64, device=p.device)
-    ops._check(ops.lib.nero_voxel_keys(ops._ptr(p), ctypes.c_longlong(n), bounds.ctypes.data_as(ctypes.c_void_p), ctypes.c_double(voxel),
-                                       ops._ptr(keys), ops._stream()), 'nero_voxel_keys')
+    ops.K('nero_voxel_keys', p, n, bounds, voxel, keys)
     skeys, order = torch.sort(keys, stable=True)            # plumbing: stable, so each voxel keeps its points in input order
     _, counts = torch.unique_consecutive(skeys, return_counts=True)
     ends = torch.cumsum(counts, 0)
     m = ends.shape[0]
     out = torch.empty(m, 3, dtype=torch.float64, device=p.device)
-    ops._check(ops.lib.nero_voxel_mean(ops._ptr(p), ops._ptr(order), ops._ptr(ends), ctypes.c_longlong(m), ops._ptr(out),
-                                       ops._stream()), 'nero_voxel_mean')
-    ops.launch_count += 2
+    ops.K('nero_voxel_mean', p, order, ends, m, out)
     return out
 
 
@@ -215,9 +198,7 @@ def nearest_dist_cuda(q, t):
     if q.shape[0] == 0 or t.shape[0] == 0:
         raise ValueError(f'nearest_dist needs two non-empty point sets, got {q.shape[0]} and {t.shape[0]} points')
     out = torch.empty(q.shape[0], dtype=torch.float32, device=q.device)
-    ops._check(ops.lib.nero_nearest_dist(ops._ptr(q), ctypes.c_longlong(q.shape[0]), ops._ptr(t), ctypes.c_longlong(t.shape[0]),
-                                         ops._ptr(out), ops._stream()), 'nero_nearest_dist')
-    ops.launch_count += 1
+    ops.K('nero_nearest_dist', q, q.shape[0], t, t.shape[0], out)
     return out
 
 

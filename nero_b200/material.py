@@ -280,12 +280,12 @@ class MaterialEngine:
                   rand_d=None if rand_d is None else rand_d.reshape(-1).contiguous(),
                   rand_s=None if rand_s is None else rand_s.reshape(-1).contiguous())
         q = self._params(st)
-        ops.mc('nero_mc_sample', q)
+        K('nero_mc_sample', q)
         K('nero_bvh_trace', self.bvh_nodes, self.bvh_tris, N, w['ORG'], 4, w['DIR'], 4, w['POSD'], w['NRMH'], MISS_DEPTH, 1)
-        ops.mc('nero_mc_classify', q)
+        K('nero_mc_classify', q)
         n_hit, n_miss = w['COUNTS'].tolist()            # the one host sync of the step
         st.update(n_hit=n_hit, n_miss=n_miss)
-        ops.mc('nero_mc_fill', q)
+        K('nero_mc_fill', q)
         A = w['ACT']
         if n_miss > 0:
             self.m_outer.forward(Mat(w['EO']), [a[:n_miss] for a in A], Mat(w['OUT_O']), None, n_miss)
@@ -293,7 +293,7 @@ class MaterialEngine:
                 self.m_human.forward(Mat(w['EH']), w['ACTH'], Mat(w['OUT_H']), None, n_miss)
         if n_hit > 0:
             self.m_inner.forward(Mat(w['EI']), [a[n_miss:] for a in A], Mat(w['OUT_I']), None, n_hit)
-        ops.mc('nero_mc_combine_fwd', q)
+        K('nero_mc_combine_fwd', q)
         self.state = st
         return w['LD'][:P].clone(), w['LS'][:P].clone(), w['LSF'][:P].clone()
 
@@ -314,7 +314,7 @@ class MaterialEngine:
         n_hit, n_miss = st['n_hit'], st['n_miss']
         q = self._params(st)
         q.set(dLD=dLD.contiguous(), dLS=dLS.contiguous(), dLSF=dLSF.contiguous())
-        ops.mc('nero_mc_combine_bwd', q)
+        K('nero_mc_combine_bwd', q)
         A, D = w['ACT'], w['dH']
         if n_miss > 0:
             ko = 144 if self.sphere else 72
@@ -327,7 +327,7 @@ class MaterialEngine:
             self.m_inner.backward(self.ws, Mat(w['DPRE_I']), Mat(w['EI']), [a[n_miss:] for a in A], D[0][n_miss:], D[1][n_miss:], None, n_hit,
                                   dX=Mat(w['dEI'], 52), dx_ncol=72, dHc=D[2][n_miss:])
         self.ws.flush()
-        ops.mc('nero_mc_dir_bwd', q)
+        K('nero_mc_dir_bwd', q)
         return w['dA'][:st['P']] + w['dA2'][:st['P']]
 
 

@@ -12,8 +12,6 @@ alone: vertices by (grid point, axis) of their edge, triangles by cube, so the s
 `material.read_ply`.  It writes the arrays as given; trimesh's default processing (the reference exports through trimesh)
 would also merge vertices at identical positions, which marching cubes only produces where a grid value equals the isovalue.
 """
-import ctypes
-
 import numpy as np
 import torch
 
@@ -38,23 +36,18 @@ def marching_cubes_cuda(u, isovalue=0.0):
     n = nx * ny * nz
     nblk = ops.ceil_div(n, _TILE)
     dev = u.device
-    iso = ctypes.c_float(float(isovalue))
     with torch.cuda.device(dev):
         blk_cnt = torch.empty(2 * nblk, dtype=torch.int32, device=dev)
         blk_off = torch.empty(2 * nblk, dtype=torch.int64, device=dev)
         totals = torch.empty(2, dtype=torch.int64, device=dev)
-        ops._check(ops.lib.nero_mcubes_count(ops._ptr(u), nx, ny, nz, iso, ops._ptr(blk_cnt), ops._ptr(blk_off), ops._ptr(totals),
-                                             ops._stream()), 'nero_mcubes_count')
-        ops.launch_count += 2
+        ops.K('nero_mcubes_count', u, nx, ny, nz, isovalue, blk_cnt, blk_off, totals, launches=2)
         V, T = totals.tolist()
         if V > _INT32_MAX or T > _INT32_MAX:
             raise RuntimeError(f'marching cubes: {V} vertices / {T} triangles do not fit int32 indices')
         verts = torch.empty(V, 3, dtype=torch.float32, device=dev)
         tris = torch.empty(T, 3, dtype=torch.int32, device=dev)
         emap = torch.empty(3 * n if V else 0, dtype=torch.int32, device=dev)
-        ops._check(ops.lib.nero_mcubes_emit(ops._ptr(u), nx, ny, nz, iso, ops._ptr(blk_off), ctypes.c_longlong(V), ctypes.c_longlong(T),
-                                            ops._ptr(emap), ops._ptr(verts), ops._ptr(tris), ops._stream()), 'nero_mcubes_emit')
-        ops.launch_count += (V > 0) + (T > 0)
+        ops.K('nero_mcubes_emit', u, nx, ny, nz, isovalue, blk_off, V, T, emap, verts, tris, launches=(V > 0) + (T > 0))
     return verts, tris
 
 

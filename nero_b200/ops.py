@@ -1,16 +1,21 @@
 """ctypes bindings of libnero_b200.so + thin tensor-level wrappers.
 
 The product path has NO fallback and no alternate backend: importing this module without the built library raises, and
-every wrapper launches a hand-written sm_90a kernel through the C ABI declared in include/nero_b200.h.  (The CPU walk of
-the host logic used by the test-suite lives in tests/dry_run_harness.py and works by substituting `lib` from outside.)
+every wrapper launches a hand-written sm_90a kernel through the C ABI declared in include/nero_b200.h.  The bindings are
+read from that header at import: every entry point gets its prototype (argtypes), every struct a ctypes.Structure with
+the header's fields.  (The CPU walk of the host logic used by the test-suite lives in tests/dry_run_harness.py and works
+by substituting `lib` from outside.)
 """
 import ctypes
 import os
+import re
 
+import numpy as np
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.environ.get('NERO_LIB') or os.path.join(_HERE, 'libnero_b200.so')   # NERO_LIB: A/B builds (profiling only)
+_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_b200.h')
 
 ACT_NONE, ACT_SOFTPLUS100, ACT_RELU, ACT_SIGMOID, ACT_EXPCLAMP = 0, 1, 2, 3, 4
 EPI_BIAS_ACT, EPI_MUL_DACT, EPI_TANGENT = 0, 1, 2
@@ -24,25 +29,116 @@ lib = ctypes.CDLL(_LIB_PATH)
 launch_count = 0  # kernels launched through the C ABI (bench.py reports it)
 
 
+def _addr(a):
+    """Address of a tensor, a Mat (its column c0), a numpy array or a ctypes struct; anything else is returned as is."""
+    if a is None:
+        return None
+    if a.__class__ is Mat:
+        return a.t.data_ptr() + 4 * a.c0
+    if isinstance(a, torch.Tensor):
+        return a.data_ptr()
+    if isinstance(a, np.ndarray):
+        return a.ctypes.data
+    if isinstance(a, ctypes.Structure):
+        return ctypes.addressof(a)
+    return a
+
+
+_CArgObject = type(ctypes.byref(ctypes.c_int()))
+
+
+class Ptr(ctypes.c_void_p):
+    """The parameter type of every pointer of the C ABI: accepts None, an int address, a tensor, a Mat, a numpy array, a
+    ctypes struct or byref(...)."""
+
+    @staticmethod
+    def from_param(a, _vp=ctypes.c_void_p, _tensor=torch.Tensor, _pass=(_CArgObject, ctypes.c_void_p)):
+        # runs for every pointer argument of every launch: the common cases first, without a further call
+        if a.__class__ is Mat:
+            return _vp(a.t.data_ptr() + 4 * a.c0)
+        if isinstance(a, _tensor):
+            return _vp(a.data_ptr())
+        if a is None or isinstance(a, _pass):
+            return a
+        return _vp(_addr(a))
+
+
+class Struct(ctypes.Structure):
+    """Base of the structs read from the header."""
+
+    def set(self, **kw):
+        for k, v in kw.items():
+            setattr(self, k, _addr(v))
+        return self
+
+
+_CTYPES = {'int': ctypes.c_int, 'unsigned int': ctypes.c_uint, 'float': ctypes.c_float, 'double': ctypes.c_double,
+           'long long': ctypes.c_longlong}
+
+
+def _parse_header(path):
+    """-> ({struct name: Struct subclass}, {entry point: argtypes}) from the typedefs and prototypes of the C header."""
+    txt = re.sub(r'/\*.*?\*/', ' ', open(path).read(), flags=re.S)
+    txt = re.sub(r'^\s*#.*$', ' ', txt, flags=re.M)
+    structs = {}
+    for body, name in re.findall(r'typedef\s+struct\s+\w*\s*\{(.*?)\}\s*(\w+)\s*;', txt, re.S):
+        fields = []
+        for decl in filter(None, (d.strip() for d in body.split(';'))):
+            first, *rest = decl.split(',')
+            base, var = re.match(r'(.*?)(\**\s*\w+\s*(?:\[\d+\])?)$', first.strip()).groups()
+            base = base.replace('const', '').strip()
+            for v in [var] + rest:
+                ptr, fname, n = re.match(r'\s*(\**)\s*(\w+)\s*(?:\[(\d+)\])?\s*$', v).groups()
+                t = ctypes.c_void_p if ptr or '*' in base else (structs.get(base) or _CTYPES[base])
+                fields.append((fname, t * int(n) if n else t))
+        structs[name] = type(name, (Struct,), {'_fields_': fields})
+    protos = {}
+    for name, params in re.findall(r'\bint\s+(nero_\w+)\s*\(([^)]*)\)\s*;', txt):
+        decls = [p.strip() for p in params.split(',') if p.strip() not in ('', 'void')]
+        protos[name] = [Ptr if '*' in p else _CTYPES[re.sub(r'\s+\w+$', '', p).replace('const', '').strip()] for p in decls]
+    return structs, protos
+
+
+STRUCTS, _PROTOS = _parse_header(_HEADER)
+for _name, _argtypes in _PROTOS.items():
+    _fn = getattr(lib, _name)
+    _fn.argtypes, _fn.restype = _argtypes, ctypes.c_int
+# nero_abi_sizeof(i) is the size of ABI_RECORDS[i]; a library built from another version of the header would read the
+# structs of every launch wrongly
+ABI_RECORDS = ('nero_chain_layer', 'nero_chain_params', 'nero_mc_params', 'nero_finish_job', 'nero_prep_job', 'nero_relight_params',
+               'nero_depth_params')
+for _i, _name in enumerate(ABI_RECORDS):
+    if lib.nero_abi_sizeof(_i) != ctypes.sizeof(STRUCTS[_name]):
+        raise ImportError(f'{_LIB_PATH}: {_name} is {lib.nero_abi_sizeof(_i)} bytes in the library but '
+                          f'{ctypes.sizeof(STRUCTS[_name])} in {_HEADER}: rebuild the library')
+ChainParams, McParams, RelightParams, DepthParams = (STRUCTS[f'nero_{n}_params'] for n in ('chain', 'mc', 'relight', 'depth'))
+_PREP_JOB, _FINISH_JOB = np.dtype(STRUCTS['nero_prep_job']), np.dtype(STRUCTS['nero_finish_job'])
+
+
 def require_cuda(dev, what='nero_b200'):
     """The kernels run on a CUDA device only: there is no CPU path to fall back to."""
     if torch.device(dev).type != 'cuda':
         raise RuntimeError(f'{what} runs on a CUDA device only (move the module with .cuda(); there is no CPU fallback)')
 
 
-def _ptr(t):
-    if t is None:
-        return ctypes.c_void_p(0)
-    return ctypes.c_void_p(t.data_ptr())
-
-
 def _stream():
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
-def _check(rc, name):
+def call(name, *args):
+    """Call entry point `name` of the library; a non-zero return code raises."""
+    rc = getattr(lib, name)(*args)
     if rc != 0:
         raise RuntimeError(f'{name} failed with code {rc}')
+
+
+def K(name, *args, launches=1):
+    """Launch entry point `name` on the current CUDA stream (appended as its last argument) and count its kernels."""
+    global launch_count
+    rc = getattr(lib, name)(*args, _stream())
+    if rc != 0:
+        raise RuntimeError(f'{name} failed with code {rc}')
+    launch_count += launches
 
 
 def npad_for(n):
@@ -88,21 +184,12 @@ class PreparedLayer:
         self.w_eff = torch.zeros(N, K, dtype=torch.float32, device=device)
 
     def prep(self):
-        global launch_count
-        w = self.weight.detach()
-        g = None if self.g is None else self.g.detach()
-        rc = lib.nero_prep_weight(_ptr(w), _ptr(g), self.K, self.row0, self.nrows, _ptr(self.kmap), ctypes.c_float(1.0),
-                                  _ptr(self.img_f), self.n_pad, _ptr(self.img_t), self.t_npad if self.img_t is not None else 0,
-                                  self.t_cols[0] if self.t_cols else 0, self.t_cols[1] if self.t_cols else 0,
-                                  _ptr(self.w_eff), self.K, _stream())
-        _check(rc, 'nero_prep_weight')
-        launch_count += 1
+        K('nero_prep_weight', self.weight, self.g, self.K, self.row0, self.nrows, self.kmap, 1.0, self.img_f, self.n_pad, self.img_t,
+          self.t_npad if self.img_t is not None else 0, self.t_cols[0] if self.t_cols else 0, self.t_cols[1] if self.t_cols else 0,
+          self.w_eff, self.K)
 
     def bias_view(self):
         return None if self.bias is None else self.bias.detach()[self.row0:self.row0 + self.nrows]
-
-
-_PREP_JOB = None
 
 
 class PrepBatch:
@@ -120,15 +207,8 @@ class PrepBatch:
         return (p(l.weight), p(l.g), p(l.kmap), p(l.img_f), p(l.img_t), p(l.w_eff))
 
     def run(self):
-        global _PREP_JOB, launch_count
         if not self.layers:
             return
-        import numpy as np
-        if _PREP_JOB is None:
-            _PREP_JOB = np.dtype([('v', 'u8'), ('g', 'u8'), ('kmap', 'u8'), ('img_f', 'u8'), ('img_t', 'u8'), ('w_eff', 'u8'), ('K', 'i4'),
-                                  ('row0', 'i4'), ('nrows', 'i4'), ('rows_pad_f', 'i4'), ('rows_pad_t', 'i4'), ('t_c0', 'i4'),
-                                  ('t_ncols', 'i4'), ('ld_weff', 'i4'), ('in_scale', 'f4'), ('pad', 'i4')])
-            assert _PREP_JOB.itemsize == 88
         key = tuple(self._ptrs(l) for l in self.layers)
         if key != self.key:
             arr = np.zeros(len(self.layers), dtype=_PREP_JOB)
@@ -137,9 +217,7 @@ class PrepBatch:
                                l.t_cols[1] if l.t_cols else 0, l.K, 1.0, 0)
             self.tab = torch.from_numpy(arr.view(np.uint8).copy()).to(self.layers[0].img_f.device)
             self.key, self.max_rows = key, int(arr['nrows'].max())
-        rc = lib.nero_prep_weight_batch(_ptr(self.tab), len(self.layers), self.max_rows, _stream())
-        _check(rc, 'nero_prep_weight_batch')
-        launch_count += 1
+        K('nero_prep_weight_batch', self.tab, len(self.layers), self.max_rows)
 
 
 class Mat:
@@ -154,9 +232,6 @@ class Mat:
     def ld(self):
         return self.t.stride(0)
 
-    def ptr(self):
-        return ctypes.c_void_p(self.t.data_ptr() + 4 * self.c0)
-
     def view(self, m=None):
         v = self.t[:, self.c0:self.c0 + self.ncol]
         return v if m is None else v[:m]
@@ -166,7 +241,6 @@ def linear(A: Mat, layer: PreparedLayer, out: Mat, ncol_out, *, transposed=False
            act_param=0.0, oscale=1.0, H: Mat = None, hscale=1.0, dact=ACT_NONE, V: Mat = None, out2: Mat = None,
            addend: Mat = None, ncol_main=None, tail: Mat = None, m_ptr=None, m_cap=None, use_bias=True):
     """out = epilogue(A @ W^T) (transposed=False) or epilogue(A @ W) restricted to t_cols (transposed=True)."""
-    global launch_count
     if ncol_main is None:
         ncol_main = ncol_out
     if transposed:
@@ -177,29 +251,9 @@ def linear(A: Mat, layer: PreparedLayer, out: Mat, ncol_out, *, transposed=False
         bias = layer.bias_view() if use_bias else None
     if m_cap is None:
         m_cap = A.t.shape[0]
-    rc = lib.nero_linear(A.ptr(), A.ld, k_valid, _ptr(img), n_pad, k_chunks, _ptr(bias), 0 if bias is None else bias.numel(), out.ptr(), out.ld, ncol_out,
-                         ctypes.c_float(oscale), mode, act, ctypes.c_float(act_param),
-                         H.ptr() if H else None, H.ld if H else 0, ctypes.c_float(hscale), dact,
-                         V.ptr() if V else None, V.ld if V else 0, out2.ptr() if out2 else None, out2.ld if out2 else 0,
-                         addend.ptr() if addend else None, addend.ld if addend else 0, ncol_main,
-                         tail.ptr() if tail else None, tail.ld if tail else 0, _ptr(m_ptr), m_cap, _stream())
-    _check(rc, 'nero_linear')
-    launch_count += 1
-
-
-_FINISH_JOB = None
-
-
-def _finish_job_dtype():
-    global _FINISH_JOB
-    if _FINISH_JOB is None:
-        import numpy as np
-        _FINISH_JOB = np.dtype([('partial', 'u8'), ('bias_partial', 'u8'), ('kmap', 'u8'), ('v', 'u8'), ('g', 'u8'), ('grad_w', 'u8'),
-                                ('grad_g', 'u8'), ('grad_b', 'u8'), ('extra_row', 'u8'), ('P', 'i4'), ('rows_partial', 'i4'),
-                                ('ld_partial', 'i4'), ('K', 'i4'), ('row0', 'i4'), ('nrows', 'i4'), ('in_scale', 'f4'),
-                                ('extra_scale', 'f4')])
-        assert _FINISH_JOB.itemsize == 104
-    return _FINISH_JOB
+    K('nero_linear', A, A.ld, k_valid, img, n_pad, k_chunks, bias, 0 if bias is None else bias.numel(), out, out.ld, ncol_out,
+      oscale, mode, act, act_param, H, H.ld if H else 0, hscale, dact, V, V.ld if V else 0, out2, out2.ld if out2 else 0,
+      addend, addend.ld if addend else 0, ncol_main, tail, tail.ld if tail else 0, m_ptr, m_cap)
 
 
 class WgradWorkspace:
@@ -246,14 +300,12 @@ class WgradWorkspace:
             self.flush()
 
     def flush(self):
-        global launch_count
         if not self.jobs:
             return
         key = tuple(self.jobs)
         hit = self._tabs.get(key)
         if hit is None:
-            import numpy as np
-            arr = np.zeros(len(self.jobs), dtype=_finish_job_dtype())
+            arr = np.zeros(len(self.jobs), dtype=_FINISH_JOB)
             for i, j in enumerate(self.jobs):
                 arr[i] = j
             if len(self._tabs) >= 64:
@@ -261,9 +313,7 @@ class WgradWorkspace:
             hit = self._tabs[key] = (torch.from_numpy(arr.view(np.uint8).copy()).to(self.device), int(arr['nrows'].max()),
                                      int(arr['K'].max()))
         tab, max_rows, max_k = hit
-        rc = lib.nero_wgrad_finish_batch(_ptr(tab), len(self.jobs), max_rows, max_k, _stream())
-        _check(rc, 'nero_wgrad_finish_batch')
-        launch_count += 1
+        K('nero_wgrad_finish_batch', tab, len(self.jobs), max_rows, max_k)
         torch._foreach_zero_(self.slots[:len(self.jobs)])     # the used accumulators are ready for the next pass
         self.jobs, self.dest, self.keep = [], set(), []
 
@@ -272,7 +322,6 @@ def wgrad(ws: WgradWorkspace, dY: Mat, n_valid, X: Mat, k_valid, layer: Prepared
           dY2: Mat = None, X2: Mat = None, m_ptr=None, m_cap=None, with_bias=True):
     """Accumulate d(weight_g, weight_v, bias) (or d(weight, bias)) of rows [row0,row0+nrows) of `layer` from
     dW_layout = dY^T X (+ dY2^T X2)."""
-    global launch_count
     if m_cap is None:
         m_cap = dY.t.shape[0]
     n_rows_pad = ceil_div(n_valid, 16) * 16
@@ -285,12 +334,9 @@ def wgrad(ws: WgradWorkspace, dY: Mat, n_valid, X: Mat, k_valid, layer: Prepared
     if not ws.defer:          # stand-alone use: the accumulator slot is zeroed per call
         partial_t.zero_()
         bias_t.zero_()
-    rc = lib.nero_wgrad(dY.ptr(), dY.ld, n_valid, X.ptr(), X.ld, k_valid,
-                        dY2.ptr() if dY2 else None, dY2.ld if dY2 else 0, X2.ptr() if X2 else None, X2.ld if X2 else 0,
-                        _ptr(partial_t), ws.ld, ws.rows, _ptr(bias_t), n_rows_pad, k_pad, P, _ptr(m_ptr),
-                        m_cap, _stream())
-    _check(rc, 'nero_wgrad')
-    launch_count += ceil_div(n_rows_pad, 128) * max(1, ceil_div(k_pad, 256))
+    K('nero_wgrad', dY, dY.ld, n_valid, X, X.ld, k_valid, dY2, dY2.ld if dY2 else 0, X2, X2.ld if X2 else 0,
+      partial_t, ws.ld, ws.rows, bias_t, n_rows_pad, k_pad, P, m_ptr, m_cap,
+      launches=ceil_div(n_rows_pad, 128) * max(1, ceil_div(k_pad, 256)))
     g = None if layer.g is None else layer.g.detach()
     w_ = layer.weight.detach()
     if ws.defer:
@@ -299,107 +345,42 @@ def wgrad(ws: WgradWorkspace, dY: Mat, n_valid, X: Mat, k_valid, layer: Prepared
                ptr(grad_b) if with_bias else 0, 0, P, ws.rows, ws.ld, layer.K, layer.row0, layer.nrows, 1.0, 0.0)
         ws.enqueue(job, (grad_w.data_ptr(), layer.row0), (w_, g))
         return
-    rc = lib.nero_wgrad_finish(_ptr(partial_t), P, ws.rows, ws.ld, _ptr(bias_t) if with_bias else None,
-                               layer.K, layer.row0, layer.nrows, _ptr(layer.kmap), ctypes.c_float(1.0),
-                               _ptr(w_), _ptr(g), _ptr(grad_w), _ptr(grad_g),
-                               _ptr(grad_b) if with_bias else None, None, ctypes.c_float(0.0), _stream())
-    _check(rc, 'nero_wgrad_finish')
-    launch_count += 1
+    K('nero_wgrad_finish', partial_t, P, ws.rows, ws.ld, bias_t if with_bias else None, layer.K, layer.row0, layer.nrows, layer.kmap,
+      1.0, w_, g, grad_w, grad_g, grad_b if with_bias else None, None, 0.0)
 
 
 def colsum(X: Mat, ncol, out, w: Mat = None, m_ptr=None, m_cap=None):
-    global launch_count
     if m_cap is None:
         m_cap = X.t.shape[0]
-    rc = lib.nero_colsum(X.ptr(), X.ld, ncol, w.ptr() if w else None, w.ld if w else 0, _ptr(m_ptr), m_cap, _ptr(out),
-                         _stream())
-    _check(rc, 'nero_colsum')
-    launch_count += 1
-
-
-def K(name, *args):
-    """Generic launcher: tensors / Mat -> device pointers, float -> c_float, int stays int, None -> NULL; the
-    current CUDA stream is appended as the last argument."""
-    global launch_count
-    conv = []
-    for a in args:
-        if a is None:
-            conv.append(ctypes.c_void_p(0))
-        elif isinstance(a, torch.Tensor):
-            conv.append(ctypes.c_void_p(a.data_ptr()))
-        elif isinstance(a, Mat):
-            conv.append(a.ptr())
-        elif isinstance(a, float):
-            conv.append(ctypes.c_float(a))
-        elif isinstance(a, ctypes._SimpleCData):
-            conv.append(a)
-        else:
-            conv.append(int(a))
-    rc = getattr(lib, name)(*conv, _stream())
-    _check(rc, name)
-    launch_count += 1
+    K('nero_colsum', X, X.ld, ncol, w, w.ld if w else 0, m_ptr, m_cap, out)
 
 
 # ------------------------------------------------------------------------------------------------ stand-alone encodings
 def positional_encoding(x, L, scale=1.0):
     """get_embedder(L, d)[0](x) (network/field.py:14-58) for d = 3 or 4 on the CUDA path: [M, d] -> [M, d(1+2L)]."""
-    global launch_count
     x = x.contiguous().float()
     M, d = x.shape
     out = torch.empty(M, d * (1 + 2 * L), device=x.device)
-    rc = lib.nero_pe(_ptr(x), d, d, M, L, ctypes.c_float(scale), _ptr(out), out.shape[1], _stream())
-    _check(rc, 'nero_pe')
-    launch_count += 1
+    K('nero_pe', x, d, d, M, L, scale, out, out.shape[1])
     return out
 
 
 def integrated_dir_enc(dirs, kappa_inv):
     """generate_ide_fn(5)(dirs, kappa_inv) (utils/ref_utils.py:53-117) on the CUDA path: [M,3], [M,1] or float -> [M,72]."""
-    global launch_count
     from .engine import upload_ide_table
     upload_ide_table()
     dirs = dirs.contiguous().float()
     M = dirs.shape[0]
     out = torch.empty(M, 72, device=dirs.device)
     if torch.is_tensor(kappa_inv):
-        k = kappa_inv.reshape(-1).contiguous().float()
-        rc = lib.nero_ide(_ptr(dirs), 3, _ptr(k), 1, ctypes.c_float(0.0), M, _ptr(out), 72, _stream())
+        K('nero_ide', dirs, 3, kappa_inv.reshape(-1).contiguous().float(), 1, 0.0, M, out, 72)
     else:
-        rc = lib.nero_ide(_ptr(dirs), 3, None, 0, ctypes.c_float(float(kappa_inv)), M, _ptr(out), 72, _stream())
-    _check(rc, 'nero_ide')
-    launch_count += 1
+        K('nero_ide', dirs, 3, None, 0, float(kappa_inv), M, out, 72)
     return out
 
 
 # ------------------------------------------------------------------------------------------------ fused MLP chain
 EK_BIAS_SOFTPLUS, EK_BIAS_RELU, EK_BIAS_GENERIC, EK_DACT_SOFTPLUS, EK_DACT_RELU, EK_DACT_NONE, EK_TANGENT = range(7)
-
-
-class _ChainLayer(ctypes.Structure):
-    _fields_ = [('wimg', ctypes.c_void_p), ('bias', ctypes.c_void_p),
-                ('save', ctypes.c_void_p), ('H', ctypes.c_void_p), ('addend', ctypes.c_void_p), ('V', ctypes.c_void_p),
-                ('out2', ctypes.c_void_p), ('tail', ctypes.c_void_p),
-                ('n_pad', ctypes.c_int), ('k_chunks', ctypes.c_int), ('n_bias', ctypes.c_int), ('ncol_out', ctypes.c_int),
-                ('ncol_main', ctypes.c_int), ('kind', ctypes.c_int), ('act', ctypes.c_int),
-                ('ld_save', ctypes.c_int), ('ldh', ctypes.c_int), ('ldadd', ctypes.c_int), ('ldv', ctypes.c_int),
-                ('ldo2', ctypes.c_int), ('ldt', ctypes.c_int),
-                ('oscale', ctypes.c_float), ('hscale', ctypes.c_float), ('act_param', ctypes.c_float),
-                ('write_a', ctypes.c_int), ('a_blocks', ctypes.c_int),
-                ('csrc', ctypes.c_void_p), ('ld_csrc', ctypes.c_int), ('pad_', ctypes.c_int)]
-
-
-class _ChainParams(ctypes.Structure):
-    _fields_ = [('A0', ctypes.c_void_p), ('lda0', ctypes.c_int), ('k_valid0', ctypes.c_int),
-                ('n_layers', ctypes.c_int), ('m_ptr', ctypes.c_void_p), ('m_cap', ctypes.c_int),
-                ('L', _ChainLayer * 10)]
-
-
-def _p(m):
-    if m is None:
-        return None
-    if isinstance(m, Mat):
-        return m.t.data_ptr() + 4 * m.c0
-    return m.data_ptr()
 
 
 def chain_layer(layer: PreparedLayer, kind, ncol_out, *, transposed=False, save: Mat = None, act=ACT_NONE, act_param=0.0, oscale=1.0,
@@ -416,13 +397,12 @@ PROFILE = None   # bench.py: list collecting (tag, event0, event1, flops_per_row
 
 def chain(A0: Mat, k_valid0, layers, m_ptr=None, m_cap=None, tag=''):
     """Run consecutive layers on each 128-row tile with the A operand kept in shared memory (k_gemm_chain.cu)."""
-    global launch_count
-    assert 1 <= len(layers) <= 10
     if m_cap is None:
         m_cap = A0.t.shape[0]
-    P = _ChainParams()
-    P.A0, P.lda0, P.k_valid0 = _p(A0), A0.ld, ceil_div(k_valid0, 4) * 4
-    P.n_layers, P.m_ptr, P.m_cap = len(layers), _p(m_ptr), m_cap
+    P = ChainParams()
+    assert 1 <= len(layers) <= len(P.L)
+    P.A0, P.lda0, P.k_valid0 = _addr(A0), A0.ld, ceil_div(k_valid0, 4) * 4
+    P.n_layers, P.m_ptr, P.m_cap = len(layers), _addr(m_ptr), m_cap
     keep = []
     for i, d in enumerate(layers):
         lay, L = d['layer'], P.L[i]
@@ -433,12 +413,12 @@ def chain(A0: Mat, k_valid0, layers, m_ptr=None, m_cap=None, tag=''):
             bias = lay.bias_view() if d['use_bias'] else None
         assert k_chunks <= 4 and d['ncol_out'] <= n_pad
         keep.append(bias)
-        L.wimg, L.bias, L.n_bias = _p(img), _p(bias), 0 if bias is None else bias.numel()
+        L.wimg, L.bias, L.n_bias = _addr(img), _addr(bias), 0 if bias is None else bias.numel()
         L.n_pad, L.k_chunks, L.ncol_out, L.ncol_main, L.kind, L.act = n_pad, k_chunks, d['ncol_out'], d['ncol_main'], d['kind'], d['act']
-        for name, key, ldname in (('save', 'save', 'ld_save'), ('H', 'H', 'ldh'), ('addend', 'addend', 'ldadd'), ('V', 'V', 'ldv'),
-                                  ('out2', 'out2', 'ldo2'), ('tail', 'tail', 'ldt'), ('csrc', 'csrc', 'ld_csrc')):
-            m = d[key]
-            setattr(L, name, _p(m))
+        for name, ldname in (('save', 'ld_save'), ('H', 'ldh'), ('addend', 'ldadd'), ('V', 'ldv'), ('out2', 'ldo2'), ('tail', 'ldt'),
+                             ('csrc', 'ld_csrc')):
+            m = d[name]
+            setattr(L, name, _addr(m))
             setattr(L, ldname, m.ld if m is not None else 0)
         L.oscale, L.hscale, L.act_param = d['oscale'], d['hscale'], d['act_param']
         L.write_a = 1 if (d['write_a'] and i + 1 < len(layers)) else 0
@@ -454,50 +434,16 @@ def chain(A0: Mat, k_valid0, layers, m_ptr=None, m_cap=None, tag=''):
             fl += 2.0 * kdim * d['ncol_out']
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-    rc = lib.nero_chain(ctypes.byref(P), _stream())
-    _check(rc, 'nero_chain')
-    launch_count += 1
+    K('nero_chain', ctypes.byref(P))
     if PROFILE is not None:
         e1.record()
         PROFILE.append((tag, e0, e1, fl, None if m_ptr is None else m_ptr.data_ptr(), m_cap))
 
 
-# ------------------------------------------------------------------------------------------------ stage II (k_mcshade.cu, k_bvh.cu)
-_vp, _ci, _cf = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
-
-
-class McParams(ctypes.Structure):
-    """Mirror of nero_mc_params (include/nero_b200.h)."""
-    _fields_ = [('pts', _vp), ('normals', _vp), ('view', _vp), ('rough', _vp), ('poses', _vp), ('rand_d', _vp), ('rand_s', _vp),
-                ('tab_d', _vp), ('tab_s', _vp), ('P', _ci), ('Sd', _ci), ('Ss', _ci), ('ggx_smith', _ci), ('sphere_dir', _ci),
-                ('human', _ci), ('org', _vp), ('dir', _vp), ('pos_depth', _vp), ('nrm_hit', _vp), ('slot', _vp), ('blk_cnt', _vp),
-                ('blk_off', _vp), ('counts', _vp), ('EO', _vp), ('ldeo', _ci), ('EH', _vp), ('ldeh', _ci), ('hhit', _vp), ('EI', _vp),
-                ('ldei', _ci), ('OUT_O', _vp), ('OUT_H', _vp), ('OUT_I', _vp), ('exp_max_o', _cf), ('exp_max_i', _cf), ('LD', _vp),
-                ('LS', _vp), ('LSF', _vp), ('dLD', _vp), ('dLS', _vp), ('dLSF', _vp), ('DPRE_O', _vp), ('DPRE_H', _vp), ('DPRE_I', _vp),
-                ('dA', _vp), ('dEO', _vp), ('dEH', _vp), ('dEI', _vp), ('dA2', _vp)]
-
-    def set(self, **kw):
-        for k, v in kw.items():
-            if isinstance(v, torch.Tensor):
-                v = v.data_ptr()
-            elif isinstance(v, Mat):
-                v = v.t.data_ptr() + 4 * v.c0
-            setattr(self, k, v)
-        return self
-
-
-def mc(name, params: McParams):
-    """Launch one of the nero_mc_* kernels on the current stream."""
-    global launch_count
-    rc = getattr(lib, name)(ctypes.byref(params), _stream())
-    _check(rc, name)
-    launch_count += 1
-
-
+# ------------------------------------------------------------------------------------------------ stage II (k_bvh.cu)
 def bvh_build(verts, tris):
     """Host BVH build through the C ABI: numpy verts [V,3] f32, tris [T,3] i32 -> (nodes uint8 [n,32], tri float32 [T,12],
     tri_ids int32 [T]) as numpy arrays ready to upload."""
-    import numpy as np
     verts = np.ascontiguousarray(verts, np.float32)
     tris = np.ascontiguousarray(tris, np.int32)
     T = tris.shape[0]
@@ -505,7 +451,5 @@ def bvh_build(verts, tris):
     tri = np.zeros((T, 12), np.float32)
     ids = np.zeros(T, np.int32)
     n = ctypes.c_int(0)
-    rc = lib.nero_bvh_build_host(verts.ctypes.data_as(_vp), verts.shape[0], tris.ctypes.data_as(_vp), T, nodes.ctypes.data_as(_vp),
-                                 tri.ctypes.data_as(_vp), ids.ctypes.data_as(_vp), ctypes.byref(n))
-    _check(rc, 'nero_bvh_build_host')
+    call('nero_bvh_build_host', verts, verts.shape[0], tris, T, nodes, tri, ids, ctypes.byref(n))
     return nodes[:n.value].copy(), tri, ids

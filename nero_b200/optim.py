@@ -7,7 +7,6 @@ re-homes all parameters as views of one flat fp32 buffer, matching the flat grad
 (`engine.Grads`), and updates it with `nero_adam_flat`.  Arithmetic follows torch's Adam (amsgrad=False) operation by
 operation; results agree with `torch.optim.Adam` to rounding.
 """
-import ctypes
 import math
 
 import torch
@@ -77,7 +76,7 @@ class FlatAdam(torch.optim.Optimizer):
         bc1 = 1.0 - b1 ** self.t
         bc2 = 1.0 - b2 ** self.t
         g = self._gather_grads()
-        ops.K('nero_adam_flat', self.flat_p, g, self.exp_avg, self.exp_avg_sq, ctypes.c_longlong(self.flat_p.numel()), float(grp['lr'] / bc1), float(b1),
+        ops.K('nero_adam_flat', self.flat_p, g, self.exp_avg, self.exp_avg_sq, self.flat_p.numel(), float(grp['lr'] / bc1), float(b1),
               float(b2), float(grp['eps']), float(1.0 / math.sqrt(bc2)), float(grp['weight_decay']))
 
     # ------------------------------------------------------------------ torch.optim.Adam-compatible checkpoints

@@ -31,7 +31,6 @@ The scene, in scene coordinates (= Blender world coordinates, z up):
     2.8-3.x's default Filmic view transform is not reproduced).
 Parity with Blender is unpinned (DESIGN.md section 2).
 """
-import ctypes
 import os
 import struct
 import zlib
@@ -331,12 +330,9 @@ class Relighter:
         if spp < 1 or max_bounces < 1 or spp_per_launch < 1:
             raise ValueError('spp, max_bounces and spp_per_launch must be positive')
         accum = torch.zeros(h * w, 4, device=self.dev)
-        q = RelightParams()
         e = self.env_d
-        for name, t in (('nodes', self.nodes), ('tris', self.tri), ('tri_ids', self.tri_ids), ('faces', self.faces),
-                        ('vmat', self.vmat_d), ('env', e['env']), ('env_p', e['p']), ('cdf_rows', e['cdf_rows']),
-                        ('cdf_cols', e['cdf_cols']), ('accum', accum), ('rays', self.rays)):
-            setattr(q, name, t.data_ptr())
+        q = ops.RelightParams().set(nodes=self.nodes, tris=self.tri, tri_ids=self.tri_ids, faces=self.faces, vmat=self.vmat_d, env=e['env'],
+                                    env_p=e['p'], cdf_rows=e['cdf_rows'], cdf_cols=e['cdf_cols'], accum=accum, rays=self.rays)
         q.pose[:] = [float(x) for x in np.asarray(pose, np.float64).reshape(12)]
         K = np.asarray(K, np.float64)
         q.K[:] = [K[0, 0], K[1, 1], K[0, 2], K[1, 2]]
@@ -344,14 +340,5 @@ class Relighter:
         q.max_bounces, q.ggx_smith, q.seed = max_bounces, self.ggx_smith, seed & 0xffffffff
         for s0 in range(0, spp, spp_per_launch):
             q.spp0, q.spp = s0, min(spp_per_launch, spp - s0)
-            ops.mc('nero_relight_render', q)
+            ops.K('nero_relight_render', q)
         return (accum / spp).reshape(h, w, 4)
-
-
-class RelightParams(ctypes.Structure):
-    """Mirror of nero_relight_params (include/nero_b200.h)."""
-    _vp, _ci, _cf = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
-    _fields_ = [('nodes', _vp), ('tris', _vp), ('tri_ids', _vp), ('faces', _vp), ('vmat', _vp), ('env', _vp), ('env_p', _vp),
-                ('cdf_rows', _vp), ('cdf_cols', _vp), ('accum', _vp), ('rays', _vp), ('pose', _cf * 12), ('K', _cf * 4),
-                ('env_w', _ci), ('env_h', _ci), ('width', _ci), ('height', _ci), ('spp0', _ci), ('spp', _ci), ('max_bounces', _ci),
-                ('ggx_smith', _ci), ('seed', ctypes.c_uint), ('pad_', _ci)]

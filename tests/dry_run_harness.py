@@ -2,13 +2,16 @@
 
 The product package has no alternate backend; this harness substitutes things from OUTSIDE:
   * `ops.lib` is wrapped: every device entry point becomes a no-op returning 0 (host-only entry points -- the BVH builder,
-    the ABI self-checks -- still run for real); the few entry points whose device-side counts drive host control flow
-    write plausible counts through the (CPU) pointers they were given;
+    the ABI self-checks -- still run for real) once its arguments pass the prototype the bindings read from the header
+    (count, then each argtype's from_param), so the walk checks the signature of every call site it reaches; the few entry
+    points whose device-side counts drive host control flow write plausible counts through the (CPU) pointers they were given;
   * `ops._stream` returns a null stream, `ops.require_cuda` accepts any device;
   * `ops.linear / chain / wgrad` are wrapped with the argument / buffer-shape assertions a wrong call sequence would trip.
 Numerical results are meaningless in this mode.
 """
 import ctypes
+
+from nero_b200 import ops
 
 
 class FakeLib:
@@ -24,6 +27,12 @@ class FakeLib:
             return real
 
         def fake(*args):
+            assert len(args) == len(real.argtypes), f'{name}: {len(args)} arguments for {len(real.argtypes)} parameters'
+            for i, (t, a) in enumerate(zip(real.argtypes, args)):
+                try:
+                    t.from_param(a)
+                except (TypeError, ValueError) as e:
+                    raise AssertionError(f'{name}: argument {i} ({a!r}) does not convert to {t.__name__}: {e}') from None
             self.calls += 1
             hook = getattr(self, '_hook_' + name, None)
             if hook is not None:
@@ -32,10 +41,10 @@ class FakeLib:
         return fake
 
     @staticmethod
-    def _poke(ptr, value):
-        addr = ptr.value if isinstance(ptr, ctypes.c_void_p) else int(ptr)
+    def _poke(ptr, value, ctype=ctypes.c_int):
+        addr = ops._addr(ptr)
         if addr:
-            ctypes.c_int.from_address(addr).value = int(value)
+            ctype.from_address(addr).value = int(value)
 
     # (rays_o, rays_d, z_vals, R, S, cnt_in, cnt_out, off_in, off_out, n_in, n_out, stream)
     def _hook_nero_ray_prepare(self, *a):
@@ -51,8 +60,16 @@ class FakeLib:
     def _hook_nero_reg_prepare(self, *a):
         self._poke(a[10], min(50, a[3] * a[4]))
 
-    def _hook_nero_mc_classify(self, q, stream):
-        p = q._obj
+    # (u, nx, ny, nz, iso, blk_cnt, blk_off, totals, stream): totals = (V, T) as long long
+    def _hook_nero_mcubes_count(self, *a):
+        self._poke(a[7], 6, ctypes.c_longlong)
+        self._poke(ops._addr(a[7]) + 8, 2, ctypes.c_longlong)
+
+    # (depth, n_views, height, width, lo, hi, blk_cnt, blk_off, total, stream)
+    def _hook_nero_depth_points_count(self, *a):
+        self._poke(a[8], min(5, a[1] * a[2] * a[3]), ctypes.c_longlong)
+
+    def _hook_nero_mc_classify(self, p, stream):
         n = p.P * (p.Sd + p.Ss)
         if p.counts:
             ctypes.c_int.from_address(p.counts).value = n // 4
@@ -60,7 +77,6 @@ class FakeLib:
 
 
 def install():
-    from nero_b200 import ops
     if isinstance(ops.lib, FakeLib):
         return ops.lib
     ops.lib = FakeLib(ops.lib)

@@ -47,13 +47,30 @@ def test_sass_uses_hopper_tensor_path():
     assert cubins and all(e.endswith('.sm_90a.cubin') for e in cubins), cubins
 
 
-def test_binding_struct_layouts_match_the_library():
-    """ctypes / numpy mirrors of the structures that cross the C ABI have the sizes the library was compiled with."""
-    import numpy as np
+def test_header_structs_match_the_library():
+    """The structs the bindings read from the header have the sizes the library was compiled with, and the numpy job
+    records have the sizes of their structs."""
     from nero_b200 import ops
     lib = ops.lib
-    assert lib.nero_abi_sizeof(0) == ctypes.sizeof(ops._ChainLayer)
-    assert lib.nero_abi_sizeof(1) == ctypes.sizeof(ops._ChainParams)
-    assert lib.nero_abi_sizeof(2) == ctypes.sizeof(ops.McParams)
-    assert lib.nero_abi_sizeof(3) == ops._finish_job_dtype().itemsize
-    assert lib.nero_abi_sizeof(4) == 88 and lib.nero_abi_sizeof(99) == -1
+    assert len(ops.ABI_RECORDS) == 7
+    for i, name in enumerate(ops.ABI_RECORDS):
+        assert lib.nero_abi_sizeof(i) == ctypes.sizeof(ops.STRUCTS[name]), name
+    assert lib.nero_abi_sizeof(len(ops.ABI_RECORDS)) == -1 and lib.nero_abi_sizeof(99) == -1
+    assert ops._PREP_JOB.itemsize == lib.nero_abi_sizeof(4) and ops._FINISH_JOB.itemsize == lib.nero_abi_sizeof(3)
+
+
+def test_every_entry_point_has_its_header_prototype():
+    """Each prototype of the header is set on the library with one argtype per parameter; a call that does not match it is
+    refused before it reaches C."""
+    import pytest
+    from nero_b200 import ops
+    txt = re.sub(r'/\*.*?\*/', ' ', open(os.path.join(ROOT, 'include', 'nero_b200.h')).read(), flags=re.S)
+    protos = dict(re.findall(r'\bint\s+(nero_[a-z0-9_]+)\s*\(([^)]*)\)', txt))
+    assert len(protos) == len(declared_symbols()) == 57
+    for name, params in protos.items():
+        n = 0 if params.strip() in ('', 'void') else params.count(',') + 1
+        fn = getattr(ops.lib, name)
+        assert fn.argtypes is not None and len(fn.argtypes) == n and fn.restype is ctypes.c_int, name
+    assert ops.lib.nero_abi_sizeof(2) > 0
+    with pytest.raises(ctypes.ArgumentError):
+        ops.lib.nero_abi_sizeof(2.0)

@@ -1,6 +1,5 @@
 """CPU: the generated marching-cubes tables (tools/gen_mc_tables.py -> nero_b200/csrc/mc_tables.cuh), the numpy oracle built on
 them (closed, consistently oriented meshes; a sphere), the PLY writer, and the argument checks of the C ABI."""
-import ctypes
 import importlib.util
 import os
 
@@ -145,15 +144,14 @@ def test_write_ply_round_trips_through_read_ply(tmp_path):
 def test_c_abi_rejects_bad_arguments_without_launching():
     from nero_b200 import ops
     lib = ops.lib
-    buf = ctypes.c_void_p(16)      # never dereferenced: the checks come first
-    iso = ctypes.c_float(0.0)
+    buf = 16      # never dereferenced: the checks come first
     for dims in ((1, 4, 4), (4, 1, 4), (4, 4, 1), (0, 4, 4)):
-        assert lib.nero_mcubes_count(buf, *dims, iso, buf, buf, buf, None) == 1
-        assert lib.nero_mcubes_emit(buf, *dims, iso, buf, ctypes.c_longlong(0), ctypes.c_longlong(0), buf, buf, buf, None) == 1
-    big = ctypes.c_longlong(2 ** 31)
-    assert lib.nero_mcubes_emit(buf, 4, 4, 4, iso, buf, big, ctypes.c_longlong(1), buf, buf, buf, None) == 1
-    assert lib.nero_mcubes_emit(buf, 4, 4, 4, iso, buf, ctypes.c_longlong(8), big, buf, buf, buf, None) == 1
-    assert lib.nero_mcubes_count(None, 4, 4, 4, iso, buf, buf, buf, None) == 1
+        assert lib.nero_mcubes_count(buf, *dims, 0.0, buf, buf, buf, None) == 1
+        assert lib.nero_mcubes_emit(buf, *dims, 0.0, buf, 0, 0, buf, buf, buf, None) == 1
+    big = 2 ** 31
+    assert lib.nero_mcubes_emit(buf, 4, 4, 4, 0.0, buf, big, 1, buf, buf, buf, None) == 1
+    assert lib.nero_mcubes_emit(buf, 4, 4, 4, 0.0, buf, 8, big, buf, buf, buf, None) == 1
+    assert lib.nero_mcubes_count(None, 4, 4, 4, 0.0, buf, buf, buf, None) == 1
 
 
 def test_marching_cubes_rejects_bad_shapes_before_touching_the_device():

@@ -114,11 +114,6 @@ def read_png(path):
     return raw[:, 1:].reshape(h, w, 4)
 
 
-def test_relight_params_layout_matches_the_library():
-    from nero_b200 import ops
-    assert ops.lib.nero_abi_sizeof(5) == ctypes.sizeof(RL.RelightParams)
-
-
 def test_relighter_has_no_cpu_path():
     verts = np.zeros((3, 3), np.float32)
     mats = {'metallic': np.zeros((3, 1)), 'roughness': np.ones((3, 1)), 'albedo': np.ones((3, 3))}
