@@ -278,19 +278,27 @@ def to_rgba8(img):
     return np.round(np.concatenate([srgb, np.clip(a, 0.0, 1.0)], -1) * 255.0).astype(np.uint8)
 
 
-def write_png_rgba(path, rgba):
-    """Write uint8 [h,w,4] as an 8-bit RGBA PNG (stdlib zlib; no image library needed)."""
-    rgba = np.ascontiguousarray(rgba, np.uint8)
-    h, w = rgba.shape[:2]
-    if rgba.shape != (h, w, 4):
-        raise ValueError(f'expected [h,w,4] uint8, got {rgba.shape}')
-    raw = np.concatenate([np.zeros((h, 1), np.uint8), rgba.reshape(h, 4 * w)], 1).tobytes()   # filter type 0 per row
+def write_png(path, img):
+    """Write uint8 [h,w,3] or [h,w,4] as an 8-bit RGB or RGBA PNG (stdlib zlib; no image library needed)."""
+    img = np.ascontiguousarray(img, np.uint8)
+    if img.ndim != 3 or img.shape[2] not in (3, 4):
+        raise ValueError(f'expected [h,w,3] or [h,w,4] uint8, got {img.shape}')
+    h, w, c = img.shape
+    raw = np.concatenate([np.zeros((h, 1), np.uint8), img.reshape(h, c * w)], 1).tobytes()   # filter type 0 per row
 
     def chunk(tag, body):
         return struct.pack('>I', len(body)) + tag + body + struct.pack('>I', zlib.crc32(tag + body) & 0xffffffff)
     with open(path, 'wb') as f:
-        f.write(b'\x89PNG\r\n\x1a\n' + chunk(b'IHDR', struct.pack('>IIBBBBB', w, h, 8, 6, 0, 0, 0)) +
+        f.write(b'\x89PNG\r\n\x1a\n' + chunk(b'IHDR', struct.pack('>IIBBBBB', w, h, 8, 6 if c == 4 else 2, 0, 0, 0)) +
                 chunk(b'IDAT', zlib.compress(raw, 6)) + chunk(b'IEND', b''))
+
+
+def write_png_rgba(path, rgba):
+    """Write uint8 [h,w,4] as an 8-bit RGBA PNG."""
+    rgba = np.asarray(rgba)
+    if rgba.ndim != 3 or rgba.shape[2] != 4:
+        raise ValueError(f'expected [h,w,4] uint8, got {rgba.shape}')
+    write_png(path, rgba)
 
 
 # ------------------------------------------------------------------------------------------------ renderer
