@@ -2,9 +2,10 @@
 #include "common.cuh"
 
 namespace nero {
-// each of k_shade.cu and k_mcshade.cu keeps its own __constant__ copy of the IDE table
+// each of k_shade.cu, k_mcshade.cu and k_envmap.cu keeps its own __constant__ copy of the IDE table
 int set_ide_table(const float* mat17x36_host);
 int set_ide_table_mc(const float* mat17x36_host);
+int set_ide_table_env(const float* mat17x36_host);
 }  // namespace nero
 
 extern "C" {
@@ -12,8 +13,9 @@ extern "C" {
 int nero_version(void) { return 100; }
 
 int nero_set_ide_table(const float* mat17x36_host) {
-  const int rc = nero::set_ide_table(mat17x36_host);
-  return rc != NERO_OK ? rc : nero::set_ide_table_mc(mat17x36_host);
+  int rc = nero::set_ide_table(mat17x36_host);
+  if (rc == NERO_OK) rc = nero::set_ide_table_mc(mat17x36_host);
+  return rc != NERO_OK ? rc : nero::set_ide_table_env(mat17x36_host);
 }
 
 int nero_abi_sizeof(int which) {

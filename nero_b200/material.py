@@ -440,6 +440,16 @@ class NeROMaterialRenderer(nn.Module):
             outs['albedo'].append(a.cpu().numpy())
         return {k: np.concatenate(v, 0) for k, v in outs.items()}
 
+    def export_lighting(self, width=1024, height=512, ssaa=4, center=(0.0, 0.0, 0.0), trans=False, max_rows=None):
+        """The outer (environment) light as a CUDA float32 [height, width, 3] map in relight's convention (nero_b200/envmap.py):
+        outer_light(IDE(d, 0)) (field.py:836-854), with sphere_direction seen from `center`; trans=True gives the map
+        tools/relight.py --trans expects.  The inner light and the human light are not part of it."""
+        from . import envmap as EM
+        c = self.shader_network.cfg
+        ol = EM.OuterLight(self.shader_network.outer_light, c['light_exp_max'],
+                           'stage2' if c['outer_light_version'] == 'sphere_direction' else None)
+        return ol.map(width, height, ssaa, 0.0, center, EM.trans_frame(trans), max_rows or EM.MAX_ROWS)
+
     def shade(self, pts, view_dirs, normals, human_poses, is_train, step=None, rands=None):
         """MCShadingNetwork.forward + material_regularization inputs (field.py:1005-1009, renderer.py:804-807).
         `rands` (optional dict rand_d, rand_s, rand_ang, rand_eps) replaces the in-function random draws."""

@@ -433,6 +433,18 @@ class NeROShapeRenderer(nn.Module):
                 outs['albedo'].append(a.cpu().numpy())
         return {k: np.concatenate(v, 0) for k, v in outs.items()}
 
+    def export_lighting(self, width=1024, height=512, ssaa=4, center=(0.0, 0.0, 0.0), trans=False, kappa_inv=(0.0, 0.1, 0.25, 0.5, 1.0),
+                        max_rows=None):
+        """Stage I's pre-filtered outer light as CUDA float32 [height, width, 3] maps in relight's convention, one per kappa_inv
+        (nero_b200/envmap.py): outer_light(IDE(d, k)) (field.py:554-589); k = 1 is the diffuse light, smaller k the specular
+        light at roughness k.  -> {k: map}.  With sphere_direction the light is seen from `center`; trans=True gives the maps
+        tools/relight.py --trans expects."""
+        from . import envmap as EM
+        c = self.color_network.cfg
+        ol = EM.OuterLight(self.color_network.outer_light, c['light_exp_max'], 'stage1' if c['sphere_direction'] else None)
+        frame = EM.trans_frame(trans)
+        return {float(k): ol.map(width, height, ssaa, float(k), center, frame, max_rows or EM.MAX_ROWS) for k in kappa_inv}
+
 
 def _material_renderer(*a, **k):
     from .material import NeROMaterialRenderer
