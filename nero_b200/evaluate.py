@@ -251,6 +251,18 @@ def read_gt_depth(root, img_id):
     return raw.astype(np.float32) / 65535 * GT_DEPTH_SCALE
 
 
+def read_gt_image(root, img_id):
+    """get_image: uint8 RGB [h,w,3] of the 8-bit <root>/<id>.png, alpha dropped."""
+    import cv2
+    path = os.path.join(root, f'{img_id}.png')
+    raw = cv2.imread(path, cv2.IMREAD_UNCHANGED)
+    if raw is None:
+        raise FileNotFoundError(path)
+    if raw.dtype != np.uint8 or raw.ndim != 3 or raw.shape[2] not in (3, 4):
+        raise ValueError(f'{path}: expected an 8-bit RGB or RGBA image, got {raw.dtype} {raw.shape}')
+    return np.ascontiguousarray(raw[..., 2::-1])
+
+
 def split_test_ids(split_path=SPLIT):
     """get_database_split(database, 'test'): the first list of the split pickle."""
     with open(split_path, 'rb') as f:
