@@ -1,5 +1,6 @@
 // Relighting path tracer (the GPU replacement of the reference's Blender Cycles render, relight.py /
-// blender_backend/relight_backend.py): a triangle mesh with per-vertex NeRO materials under an equirectangular environment map.
+// blender_backend/relight_backend.py): a triangle mesh with per-vertex or UV-textured NeRO materials under an equirectangular
+// environment map.  The two material sources differ only in surface(); relight_kernel is one path loop instantiated for each.
 //
 // One thread per pixel loops over the sample indices [spp0, spp0 + spp) in order and adds each camera path's radiance into a
 // per-pixel fp32 running sum (rgb, hit count).  Every random number is a hash of (seed, pixel, sample, bounce, dim)
@@ -10,6 +11,7 @@
 #include "bvh_traverse.cuh"
 #include "common.cuh"
 #include "math_relight.cuh"
+#include "../../include/nero_relight_tex.h"
 
 namespace nero {
 
@@ -20,7 +22,8 @@ struct SurfHit {
   float albedo[3], metallic, alpha;
 };
 
-__device__ __forceinline__ void surface(const nero_relight_params& q, const BvhHit& h, const float* o, const float* d, SurfHit& s) {
+// hit point and flat normal, shared by both material sources
+__device__ __forceinline__ void hit_geometry(const nero_relight_params& q, const BvhHit& h, const float* o, const float* d, SurfHit& s) {
   const float4* tris = reinterpret_cast<const float4*>(q.tris);
   const float4 e1 = __ldg(tris + 3 * h.tri + 1), e2 = __ldg(tris + 3 * h.tri + 2);
   // marching-cubes meshes are wound with cross(e1, e2) pointing into the solid: the outward normal is its negation
@@ -28,6 +31,16 @@ __device__ __forceinline__ void surface(const nero_relight_params& q, const BvhH
   normalize3(n, n);
   if (rl_dot(n, d) > 0.f) { n[0] = -n[0]; n[1] = -n[1]; n[2] = -n[2]; }   // two-sided
   for (int k = 0; k < 3; ++k) { s.p[k] = o[k] + h.t * d[k]; s.n[k] = n[k]; }
+}
+
+struct VertexMaterials {};          // q.vmat [V,8] rows, interpolated barycentrically
+struct TexMaterials {              // include/nero_relight_tex.h: vt [n_uv,2], ft [T,3], tex [h,w,8]
+  const float2* vt; const int* ft; const float4* tex; int w, h;
+};
+
+__device__ __forceinline__ void surface(const nero_relight_params& q, VertexMaterials, const BvhHit& h, const float* o, const float* d,
+                                        SurfHit& s) {
+  hit_geometry(q, h, o, d, s);
   const int f = __ldg(q.tri_ids + h.tri);
   const float w0 = 1.0f - h.u - h.v;
   const float4* vm = reinterpret_cast<const float4*>(q.vmat);
@@ -45,12 +58,52 @@ __device__ __forceinline__ void surface(const nero_relight_params& q, const BvhH
   s.alpha = r * r;
 }
 
+__device__ __forceinline__ int wrap(int i, int n) {   // positive modulo: the repeat address mode
+  i %= n;
+  return i < 0 ? i + n : i;
+}
+
+// Textured materials: uv interpolated like the per-vertex rows, then a bilinear, wrapping fetch of the [h,w,8] texel rows with
+// v = 0 at the bottom image row (row h-1).  alpha is the filtered roughness itself: the texture export stores the rescaled
+// roughness NeRO's shading takes, not its square root.
+__device__ __forceinline__ void surface(const nero_relight_params& q, const TexMaterials& m, const BvhHit& h, const float* o,
+                                        const float* d, SurfHit& s) {
+  hit_geometry(q, h, o, d, s);
+  const int f = __ldg(q.tri_ids + h.tri);
+  const float w0 = 1.0f - h.u - h.v;
+  float2 t[3];
+  for (int c = 0; c < 3; ++c) t[c] = __ldg(m.vt + __ldg(m.ft + 3 * f + c));
+  const float uvx = w0 * t[0].x + h.u * t[1].x + h.v * t[2].x;
+  const float uvy = w0 * t[0].y + h.u * t[1].y + h.v * t[2].y;
+  const float sx = uvx * float(m.w) - 0.5f, sy = (1.0f - uvy) * float(m.h) - 0.5f;
+  const float x0 = floorf(sx), y0 = floorf(sy);
+  const float fx = sx - x0, fy = sy - y0;
+  const int ix = wrap(int(x0), m.w), iy = wrap(int(y0), m.h);
+  const int ix1 = ix + 1 == m.w ? 0 : ix + 1, iy1 = iy + 1 == m.h ? 0 : iy + 1;
+  const size_t r0 = size_t(iy) * m.w, r1 = size_t(iy1) * m.w;
+  const size_t tap[4] = {r0 + ix, r0 + ix1, r1 + ix, r1 + ix1};
+  float4 a[4];
+  float r[4];
+  for (int k = 0; k < 4; ++k) {
+    a[k] = __ldg(m.tex + 2 * tap[k]);
+    r[k] = __ldg(reinterpret_cast<const float*>(m.tex + 2 * tap[k] + 1));
+  }
+  auto lerp = [](float p, float q_, float w) { return p + w * (q_ - p); };
+  auto bilerp = [&](float c00, float c10, float c01, float c11) { return lerp(lerp(c00, c10, fx), lerp(c01, c11, fx), fy); };
+  s.albedo[0] = bilerp(a[0].x, a[1].x, a[2].x, a[3].x);
+  s.albedo[1] = bilerp(a[0].y, a[1].y, a[2].y, a[3].y);
+  s.albedo[2] = bilerp(a[0].z, a[1].z, a[2].z, a[3].z);
+  s.metallic = bilerp(a[0].w, a[1].w, a[2].w, a[3].w);
+  s.alpha = bilerp(r[0], r[1], r[2], r[3]);
+}
+
 __device__ __forceinline__ float mis(float a, float b) {   // power heuristic a^2 / (a^2 + b^2)
   const float a2 = a * a;
   return a2 / (a2 + b * b);
 }
 
-__global__ void __launch_bounds__(128) relight_kernel(const nero_relight_params q) {
+template <class Materials>
+__global__ void __launch_bounds__(128) relight_kernel(const nero_relight_params q, const Materials mat) {
   const int x = blockIdx.x * 16 + (threadIdx.x & 15), y = blockIdx.y * 8 + (threadIdx.x >> 4);
   if (x >= q.width || y >= q.height) return;
   const uint32_t pix = uint32_t(y) * uint32_t(q.width) + uint32_t(x);
@@ -78,7 +131,7 @@ __global__ void __launch_bounds__(128) relight_kernel(const nero_relight_params 
     float L[3] = {0.f, 0.f, 0.f}, thr[3] = {1.f, 1.f, 1.f};
     for (int b = 0; b < q.max_bounces; ++b) {
       SurfHit sh;
-      surface(q, h, o, d, sh);
+      surface(q, mat, h, o, d, sh);
       const float v[3] = {-d[0], -d[1], -d[2]};
       float po[3];
       for (int k = 0; k < 3; ++k) po[k] = sh.p[k] + kRelightEps * sh.n[k];
@@ -147,19 +200,33 @@ __global__ void __launch_bounds__(128) relight_kernel(const nero_relight_params 
   if (q.rays) atomicAdd(q.rays, rays);
 }
 
+// every check of a launch except those of the material source
+bool scene_ok(const nero_relight_params& q) {
+  if (!q.nodes || !q.tris || !q.tri_ids || !q.faces || !q.env || !q.env_p || !q.cdf_rows || !q.cdf_cols || !q.accum) return false;
+  return q.env_w >= 1 && q.env_h >= 1 && q.width >= 1 && q.height >= 1 && q.spp0 >= 0 && q.spp >= 0 && q.max_bounces >= 1;
+}
+
+template <class Materials>
+int launch(const nero_relight_params& q, const Materials& m, void* stream) {
+  if (q.spp == 0) return NERO_OK;
+  const dim3 grid((q.width + 15) / 16, (q.height + 7) / 8);
+  relight_kernel<<<grid, 128, 0, (cudaStream_t)stream>>>(q, m);
+  NERO_LAUNCH_CHECK();
+  return NERO_OK;
+}
+
 }  // namespace
 
 extern "C" int nero_relight_render(const nero_relight_params* p, void* stream) {
-  if (!p) return NERO_ERR_ARG;
-  const nero_relight_params& q = *p;
-  if (!q.nodes || !q.tris || !q.tri_ids || !q.faces || !q.vmat || !q.env || !q.env_p || !q.cdf_rows || !q.cdf_cols || !q.accum)
-    return NERO_ERR_ARG;
-  if (q.env_w < 1 || q.env_h < 1 || q.width < 1 || q.height < 1 || q.spp0 < 0 || q.spp < 0 || q.max_bounces < 1) return NERO_ERR_ARG;
-  if (q.spp == 0) return NERO_OK;
-  const dim3 grid((q.width + 15) / 16, (q.height + 7) / 8);
-  relight_kernel<<<grid, 128, 0, (cudaStream_t)stream>>>(q);
-  NERO_LAUNCH_CHECK();
-  return NERO_OK;
+  if (!p || !p->vmat || !scene_ok(*p)) return NERO_ERR_ARG;
+  return launch(*p, VertexMaterials{}, stream);
+}
+
+extern "C" int nero_relight_render_textured(const nero_relight_params* p, const float* vt, const int* ft, int n_uv, const float* tex,
+                                            int tex_w, int tex_h, void* stream) {
+  if (!p || p->vmat || !scene_ok(*p) || !vt || !ft || !tex || n_uv < 1 || tex_w < 1 || tex_h < 1) return NERO_ERR_ARG;
+  const TexMaterials m{reinterpret_cast<const float2*>(vt), ft, reinterpret_cast<const float4*>(tex), tex_w, tex_h};
+  return launch(*p, m, stream);
 }
 
 }  // namespace nero

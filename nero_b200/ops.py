@@ -19,6 +19,7 @@ _HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_b200.h')
 _TEXMAP_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_texmap.h')   # same library, plain-argument entry points
 _ENVMAP_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_envmap.h')   # same library, plain-argument entry points
 _METRICS_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_metrics.h')  # same library, plain-argument entry points
+_RELIGHT_TEX_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_relight_tex.h')   # same library, plain arguments
 
 ACT_NONE, ACT_SOFTPLUS100, ACT_RELU, ACT_SIGMOID, ACT_EXPCLAMP = 0, 1, 2, 3, 4
 EPI_BIAS_ACT, EPI_MUL_DACT, EPI_TANGENT = 0, 1, 2
@@ -106,8 +107,9 @@ STRUCTS, _PROTOS = _parse_header(_HEADER)
 TEXMAP_PROTOS = _parse_header(_TEXMAP_HEADER)[1]
 ENVMAP_PROTOS = _parse_header(_ENVMAP_HEADER)[1]
 METRICS_PROTOS = _parse_header(_METRICS_HEADER)[1]
+RELIGHT_TEX_PROTOS = _parse_header(_RELIGHT_TEX_HEADER)[1]
 for _name, _argtypes in (list(_PROTOS.items()) + list(TEXMAP_PROTOS.items()) + list(ENVMAP_PROTOS.items()) +
-                         list(METRICS_PROTOS.items())):
+                         list(METRICS_PROTOS.items()) + list(RELIGHT_TEX_PROTOS.items())):
     _fn = getattr(lib, _name)
     _fn.argtypes, _fn.restype = _argtypes, ctypes.c_int
 # nero_abi_sizeof(i) is the size of ABI_RECORDS[i]; a library built from another version of the header would read the

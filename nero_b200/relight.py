@@ -14,6 +14,17 @@ The scene, in scene coordinates (= Blender world coordinates, z up):
   * Materials: the exported per-vertex values decoded with srgb_to_linear (undoing the export gamma, as Blender's
     vertex-colour path does), interpolated barycentrically at the hit point.  The BRDF's roughness argument is
     alpha = (decoded roughness)^2, the value NeRO's shading functions take (network/field.py:794, 893).
+  * Textured materials (the textured OBJ of tools/extract_materials_texture_map.py, read by load_textured_obj): the texels
+    decoded with srgb_to_linear(k / 255).  At a hit with barycentrics (u, v), w0 = 1 - u - v:
+      uv = w0 uv0 + u uv1 + v uv2 in fp32, as the per-vertex rows are interpolated;
+      s = uv.x W - 1/2, t = (1 - uv.y) H - 1/2 for a W x H texture whose row 0 is the top row of the image file (the
+      OBJ / Blender convention, v = 0 at the bottom row; texmap.obj_text stores 1 - v_atlas, so this is the baked texel);
+      x0 = floor(s), fx = s - x0, likewise y0, fy; the four taps wrap (repeat, positive modulo);
+      bilinear in lerp form a + f (b - a) per channel, along x first, so a constant texture gives its value exactly.
+    albedo and metallic are the filtered values and alpha = the filtered roughness, NOT squared: the texture export stores
+    the rescaled roughness NeRO's shading takes (predict_materials_n2m, network/field.py:925-932), the per-vertex export its
+    square root.  There is no mip-mapping: the per-pixel jitter averages the texture over the pixel footprint as samples
+    accumulate, and a texture minified to several texels per pixel aliases at low sample counts.
   * BRDF: NeRO's stage-II model (the terms the materials were fitted under), not Blender's Principled BSDF:
     albedo (1-m)/pi + F D G / (4 NoV NoL), F0 = 0.04 (1-m) + m albedo, Schlick F, NeRO's D (with its +1e-4) and
     G = 'schlick' or 'ggx_smith' (nero_b200/csrc/math_relight.cuh, math_mc.cuh).
@@ -89,6 +100,147 @@ def vertex_material_table(materials):
     t = np.zeros((a.shape[0], 8), np.float32)
     t[:, :3], t[:, 3], t[:, 4] = a, m, r
     return t
+
+
+class UVMaterials:
+    """Materials as UV textures: vt [N,2] float uv, ft [T,3] int indices into vt (one row per triangle of the mesh), and
+    linear (decoded) maps with row 0 at the top of the image: albedo [H,W,3], metallic [H,W] or [H,W,1], roughness [H,W] or
+    [H,W,1] (the rescaled roughness, the BRDF's alpha itself)."""
+
+    def __init__(self, vt, ft, albedo, metallic, roughness):
+        self.vt = np.ascontiguousarray(vt, np.float32)
+        self.ft = np.ascontiguousarray(ft, np.int32)
+        self.albedo = np.asarray(albedo, np.float32)
+        self.metallic = np.asarray(metallic, np.float32)
+        self.roughness = np.asarray(roughness, np.float32)
+        if self.vt.ndim != 2 or self.vt.shape[1] != 2 or self.vt.shape[0] < 1:
+            raise ValueError(f'vt has shape {self.vt.shape}; expected [N,2] with N >= 1')
+        if self.ft.ndim != 2 or self.ft.shape[1] != 3:
+            raise ValueError(f'ft has shape {self.ft.shape}; expected [T,3]')
+        if self.ft.size and (self.ft.min() < 0 or self.ft.max() >= self.vt.shape[0]):
+            raise ValueError(f'ft indexes [{self.ft.min()}, {self.ft.max()}] outside the {self.vt.shape[0]} uv vertices')
+        if self.albedo.ndim != 3 or self.albedo.shape[2] != 3 or min(self.albedo.shape[:2]) < 1:
+            raise ValueError(f'albedo map has shape {self.albedo.shape}; expected [H,W,3]')
+        hw = self.albedo.shape[:2]
+        for k in ('metallic', 'roughness'):
+            a = getattr(self, k)
+            if a.shape not in (hw, hw + (1,)):
+                raise ValueError(f'{k} map has shape {a.shape}; the albedo map is {hw}')
+        if not all(np.isfinite(a).all() for a in (self.vt, self.albedo, self.metallic, self.roughness)):
+            raise ValueError('UV materials hold non-finite values')
+
+    def texel_table(self):
+        """[H,W,8] float32 texel rows (albedo rgb, metallic, roughness, 0, 0, 0), the layout nero_relight_render_textured
+        reads."""
+        H, W = self.albedo.shape[:2]
+        t = np.zeros((H, W, 8), np.float32)
+        t[..., :3], t[..., 3], t[..., 4] = self.albedo, self.metallic.reshape(H, W), self.roughness.reshape(H, W)
+        return t
+
+
+def _obj_error(path, what):
+    return ValueError(f'{path}: {what}')
+
+
+def _obj_index(tok, n, path, lineno, what):
+    try:
+        i = int(tok)
+    except ValueError:
+        raise _obj_error(path, f'line {lineno}: {what} index {tok!r} is not an integer') from None
+    if not 1 <= i <= n:
+        raise _obj_error(path, f'line {lineno}: {what} index {i} is out of range [1, {n}]')
+    return i - 1
+
+
+def _read_map(path, channels):
+    """An 8-bit image file -> float32 [H,W,len(channels)] decoded with srgb_to_linear(k / 255); channels index RGB."""
+    import cv2
+    if not os.path.isfile(path):
+        raise ValueError(f'{path}: texture file is missing')
+    img = cv2.imread(path, cv2.IMREAD_COLOR)
+    if img is None:
+        raise ValueError(f'{path}: not an image OpenCV can read')
+    rgb = img[..., ::-1]
+    return srgb_to_linear(rgb[..., list(channels)].astype(np.float64) / 255).astype(np.float32)
+
+
+def load_textured_obj(path):
+    """Read the textured OBJ of tools/extract_materials_texture_map.py (or the reference's) ->
+    (verts [V,3] float32, tris [T,3] int32, vt [N,2] float32 as written in the file, ft [T,3] int32,
+    maps {'metallic' [H,W,1], 'roughness' [H,W,1], 'albedo' [H,W,3]} float32 linear, row 0 at the top).
+
+    The OBJ gives v, vt, triangles `f a/b c/d e/f` (the a/b/n form too; normals are ignored) and `mtllib`; the MTL's
+    `map_Kd` names the albedo file, and the metallic and roughness files are named alike with feat1_ and feat2_ in place of
+    feat0_.  Images are read with OpenCV (PNG or JPEG); metallic and roughness come from the red channel.  Every value is
+    decoded with srgb_to_linear(k / 255), as load_materials decodes its arrays.  Anything else raises ValueError naming the
+    file: faces that are not triangles or lack uv indices, indices out of range, non-finite values, a missing MTL or texture
+    file, or maps of different sizes."""
+    verts, uvs, faces, mtllib = [], [], [], None
+    with open(path) as f:
+        lines = f.read().splitlines()
+    for lineno, line in enumerate(lines, 1):
+        tok = line.split()
+        if not tok:
+            continue
+        if tok[0] == 'v':
+            verts.append((lineno, tok[1:4]))
+        elif tok[0] == 'vt':
+            uvs.append((lineno, tok[1:3]))
+        elif tok[0] == 'f':
+            faces.append((lineno, tok[1:]))
+        elif tok[0] == 'mtllib' and mtllib is None:
+            mtllib = line.strip()[len('mtllib'):].strip()
+
+    def floats(rows, k, what):
+        out = np.zeros((len(rows), k), np.float64)
+        for i, (lineno, t) in enumerate(rows):
+            try:
+                if len(t) < k:
+                    raise ValueError
+                out[i] = [float(x) for x in t[:k]]
+            except ValueError:
+                raise _obj_error(path, f'line {lineno}: {what} needs {k} numbers') from None
+        if not np.isfinite(out).all():
+            raise _obj_error(path, f'non-finite {what} coordinates')
+        return out
+    V, N = floats(verts, 3, 'vertex'), floats(uvs, 2, 'texture vertex')
+    tris = np.zeros((len(faces), 3), np.int32)
+    ft = np.zeros((len(faces), 3), np.int32)
+    for i, (lineno, corners) in enumerate(faces):
+        if len(corners) != 3:
+            raise _obj_error(path, f'line {lineno}: a face with {len(corners)} corners (only triangles are supported)')
+        for c, corner in enumerate(corners):
+            parts = corner.split('/')
+            if len(parts) < 2 or not parts[1]:
+                raise _obj_error(path, f'line {lineno}: face corner {corner!r} has no uv index')
+            tris[i, c] = _obj_index(parts[0], V.shape[0], path, lineno, 'vertex')
+            ft[i, c] = _obj_index(parts[1], N.shape[0], path, lineno, 'uv')
+    if not faces:
+        raise _obj_error(path, 'no faces')
+    if mtllib is None:
+        raise _obj_error(path, 'no mtllib line')
+    mtl_path = os.path.join(os.path.dirname(path), mtllib)
+    if not os.path.isfile(mtl_path):
+        raise ValueError(f'{mtl_path}: material file is missing')
+    map_kd = None
+    with open(mtl_path) as f:
+        for line in f:
+            if line.split()[:1] == ['map_Kd']:
+                map_kd = line.strip()[len('map_Kd'):].strip()
+                break
+    if map_kd is None:
+        raise ValueError(f'{mtl_path}: no map_Kd line')
+    name = os.path.basename(map_kd)
+    if 'feat0_' not in name:
+        raise ValueError(f'{mtl_path}: map_Kd {map_kd!r} is not named feat0_*, so the metallic and roughness maps cannot be found')
+    base = os.path.join(os.path.dirname(mtl_path), os.path.dirname(map_kd))
+    files = {'albedo': os.path.join(base, name), 'metallic': os.path.join(base, name.replace('feat0_', 'feat1_', 1)),
+             'roughness': os.path.join(base, name.replace('feat0_', 'feat2_', 1))}
+    maps = {k: _read_map(files[k], (0, 1, 2) if k == 'albedo' else (0,)) for k in MATERIAL_NAMES}
+    sizes = {k: m.shape[:2] for k, m in maps.items()}
+    if len(set(sizes.values())) != 1:
+        raise ValueError(f'{path}: texture maps differ in size: ' + ', '.join(f'{files[k]} {sizes[k][1]}x{sizes[k][0]}' for k in MATERIAL_NAMES))
+    return V.astype(np.float32), tris, N.astype(np.float32), ft, maps
 
 
 # ------------------------------------------------------------------------------------------------ environment maps
@@ -303,10 +455,11 @@ def write_png_rgba(path, rgba):
 
 # ------------------------------------------------------------------------------------------------ renderer
 class Relighter:
-    """A mesh with per-vertex materials under one environment map, resident on the GPU.
+    """A mesh with per-vertex or UV-textured materials under one environment map, resident on the GPU.
 
     verts [V,3] (scene coordinates), tris [T,3]; materials = linear (decoded) {'metallic' [V,1], 'roughness' [V,1],
-    'albedo' [V,3]} (see load_materials); env [H,W,3] radiance (load_env_map); geometry_type 'schlick' or 'ggx_smith'."""
+    'albedo' [V,3]} (see load_materials) or a UVMaterials (see load_textured_obj); env [H,W,3] radiance (load_env_map);
+    geometry_type 'schlick' or 'ggx_smith'."""
 
     def __init__(self, verts, tris, materials, env, geometry_type='schlick', device='cuda'):
         import torch
@@ -317,13 +470,23 @@ class Relighter:
         self.dev = torch.device(device)
         self.verts = np.ascontiguousarray(verts, np.float32)
         self.tris = np.ascontiguousarray(tris, np.int32)
-        self.vmat = vertex_material_table(materials)
-        if self.vmat.shape[0] != self.verts.shape[0]:
-            raise ValueError(f'{self.vmat.shape[0]} material rows for {self.verts.shape[0]} vertices')
+        up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(self.dev)
+        self.uv = materials if isinstance(materials, UVMaterials) else None
+        if self.uv is not None:
+            if self.uv.ft.shape != self.tris.shape:
+                raise ValueError(f'ft has shape {self.uv.ft.shape} for tris of shape {self.tris.shape}')
+            self.vmat, self.vmat_d = None, None
+            self.tex = self.uv.texel_table()
+            self.vt_d, self.ft_d, self.tex_d = up(self.uv.vt), up(self.uv.ft), up(self.tex)
+        else:
+            self.vmat = vertex_material_table(materials)
+            if self.vmat.shape[0] != self.verts.shape[0]:
+                raise ValueError(f'{self.vmat.shape[0]} material rows for {self.verts.shape[0]} vertices')
         self.ggx_smith = 1 if geometry_type == 'ggx_smith' else 0
         nodes, tri, ids = ops.bvh_build(self.verts, self.tris)
-        up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(self.dev)
-        self.nodes, self.tri, self.tri_ids, self.faces, self.vmat_d = up(nodes), up(tri), up(ids), up(self.tris), up(self.vmat)
+        self.nodes, self.tri, self.tri_ids, self.faces = up(nodes), up(tri), up(ids), up(self.tris)
+        if self.uv is None:
+            self.vmat_d = up(self.vmat)
         self.tables = env_tables(env)
         self.env_h, self.env_w = self.tables['p'].shape
         self.env_d = {k: up(v) for k, v in self.tables.items()}
@@ -348,5 +511,9 @@ class Relighter:
         q.max_bounces, q.ggx_smith, q.seed = max_bounces, self.ggx_smith, seed & 0xffffffff
         for s0 in range(0, spp, spp_per_launch):
             q.spp0, q.spp = s0, min(spp_per_launch, spp - s0)
-            ops.K('nero_relight_render', q)
+            if self.uv is None:
+                ops.K('nero_relight_render', q)
+            else:
+                ops.K('nero_relight_render_textured', q, self.vt_d, self.ft_d, self.vt_d.shape[0], self.tex_d, self.tex.shape[1],
+                      self.tex.shape[0])
         return (accum / spp).reshape(h, w, 4)

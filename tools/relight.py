@@ -2,6 +2,10 @@
 
     python tools/relight.py --mesh data/meshes/bell_shape-300000.ply --material data/materials/bell_material-100000 \
         --hdr data/hdr/neon_photostudio_4k.exr --name bell [--trans]
+    python tools/relight.py --obj n2m_test/mesh_0.obj --hdr data/hdr/neon_photostudio_4k.exr --name bell [--trans]
+
+The materials are per-vertex (--mesh with --material, as tools/extract_materials.py writes them) or UV textures (--obj, the
+textured OBJ of tools/extract_materials_texture_map.py with its MTL and feat{0,1,2} images); exactly one form is accepted.
 
 Renders frames k = 0 .. num-1 of the reference's turntable (blender_backend/relight_backend.py) to data/relight/<name>/<k>.png
 (RGBA8, transparent background); frames that already exist are skipped.  The scene -- geometry, materials, BRDF, cameras,
@@ -16,10 +20,11 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 
-def main(argv=None):
+def parse(argv=None):
     parser = argparse.ArgumentParser(description=__doc__.split('\n')[0])
-    parser.add_argument('--mesh', type=str, required=True)
-    parser.add_argument('--material', type=str, required=True, help='directory with metallic.npy, roughness.npy, albedo.npy')
+    parser.add_argument('--mesh', type=str, default=None)
+    parser.add_argument('--material', type=str, default=None, help='directory with metallic.npy, roughness.npy, albedo.npy')
+    parser.add_argument('--obj', type=str, default=None, help='textured OBJ (with its MTL and feat0/1/2 texture images)')
     parser.add_argument('--hdr', type=str, required=True, help='environment map (.hdr or .exr)')
     parser.add_argument('--name', type=str, required=True)
     parser.add_argument('--trans', action='store_true', default=False, help='rotate the mesh by +90 degrees about x')
@@ -34,17 +39,32 @@ def main(argv=None):
     parser.add_argument('--geometry', choices=('schlick', 'ggx_smith'), default='schlick')
     parser.add_argument('--seed', type=int, default=0)
     flags = parser.parse_args(argv)
+    if flags.obj is not None:
+        if flags.mesh is not None or flags.material is not None:
+            parser.error('--obj cannot be combined with --mesh / --material')
+    elif flags.mesh is None or flags.material is None:
+        parser.error('give --mesh with --material, or --obj')
+    return flags
+
+
+def main(argv=None):
+    flags = parse(argv)
 
     import numpy as np
     import torch
     from nero_b200.material import read_ply
-    from nero_b200.relight import (MESH_TRANS, Relighter, blender_default_K, load_env_map, load_materials, relight_poses, to_rgba8,
-                                   write_png_rgba)
+    from nero_b200.relight import (MESH_TRANS, Relighter, UVMaterials, blender_default_K, load_env_map, load_materials,
+                                   load_textured_obj, relight_poses, to_rgba8, write_png_rgba)
 
-    verts, tris = read_ply(flags.mesh)
+    if flags.obj is not None:
+        verts, tris, vt, ft, maps = load_textured_obj(flags.obj)
+        materials = UVMaterials(vt, ft, maps['albedo'], maps['metallic'], maps['roughness'])
+    else:
+        verts, tris = read_ply(flags.mesh)
+        materials = load_materials(flags.material)
     if flags.trans:
         verts = (verts.astype(np.float64) @ MESH_TRANS.T).astype(np.float32)
-    relighter = Relighter(verts, tris, load_materials(flags.material), load_env_map(flags.hdr), flags.geometry)
+    relighter = Relighter(verts, tris, materials, load_env_map(flags.hdr), flags.geometry)
     K = blender_default_K(flags.height, flags.width)
     poses = relight_poses(flags.num, flags.azimuth, flags.elevation, flags.cam_dist)
     out_dir = os.path.join('data', 'relight', flags.name)
