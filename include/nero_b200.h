@@ -78,9 +78,11 @@ int nero_chain(const void* chain_params_host, void* stream);
 int nero_row_axpy(const float* a, int lda, const float* X, int ldx, float* Y, int ldy, int ncol, const int* m_ptr, int m_cap, void* stream);
 
 /* ---- weight gradients -------------------------------------------------------------------------------------
- * partial += dY^T X (+ dY2^T X2): P CTAs per 128-row output tile each contract a slice of the sample rows and add their tile
- * into their own slice p of the [P x rows_partial x ld_partial] fp32 accumulator `partial` (and the column sums of dY into
- * `bias_partial` [P x rows_partial]); the caller zeroes both before the call.  No atomics: the result is the same every run.
+ * partial = dY^T X (+ dY2^T X2) split over sample rows: P CTAs per 128-row output tile each contract a slice of the sample
+ * rows and store their tile into their own slice p of the [P x rows_partial x ld_partial] fp32 array `partial` (and the
+ * column sums of dY into `bias_partial` [P x rows_partial]).  Every slice's rows [0, 128 * ceil(n_rows_pad / 128)) (clipped
+ * to rows_partial) x columns [0, k_pad) are stored, zeros included, so the caller need not initialise either array.  No
+ * atomics: the result is the same every run.
  * Replaces the autograd weight-gradient GEMMs; nero_wgrad_finish is then called with the same P. */
 int nero_wgrad(const float* dY, int ldy, int n_valid, const float* X, int ldx, int k_valid,
                const float* dY2, int ldy2, const float* X2, int ldx2,

@@ -69,6 +69,16 @@ __device__ __forceinline__ void bulk_copy_g2s(void* smem_dst, const void* gmem_s
       : "memory");
 }
 
+// ------------------------------------------------------------------ per-thread async copy global -> shared (LDGSTS)
+// 16 bytes; the first src_bytes (0..16) come from gmem_src (16-byte aligned), the rest is zero-filled.  Through L2 only (.cg).
+__device__ __forceinline__ void cp_async16(uint32_t smem_dst, const void* gmem_src, uint32_t src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_dst), "l"(gmem_src), "r"(src_bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+// the thread's own copies of all but the newest N committed groups have landed (and are visible to it)
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
 // ------------------------------------------------------------------ wgmma
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }

@@ -266,19 +266,20 @@ def linear(A: Mat, layer: PreparedLayer, out: Mat, ncol_out, *, transposed=False
 
 
 class WgradWorkspace:
-    """Accumulators of the weight-gradient GEMMs.  nero_wgrad splits the sample rows over `P` CTAs per output tile; CTA p adds
-    its tile into slice p of a [P, rows, ld] fp32 accumulator, and the finish kernel sums the slices in a fixed order, so the
-    gradients are the same every run (no floating-point atomics).
-    With `defer` set (the engines do), every nero_wgrad launch gets its own accumulator slot and its weight-norm chain rule is
-    queued; `flush()` runs all queued jobs in ONE nero_wgrad_finish_batch launch and re-zeroes the used slots (one memset).
+    """Split-K slices of the weight-gradient GEMMs.  nero_wgrad splits the sample rows over `P` CTAs per output tile; CTA p
+    stores its tile into slice p of a [P, rows, ld] fp32 slot, and the finish kernel sums the slices in a fixed order, so the
+    gradients are the same every run (no floating-point atomics).  Every launch stores its whole window of every slice
+    (zeros where a CTA has no samples) and the finish reads only that window, so slots are never zeroed.
+    With `defer` set (the engines do), every nero_wgrad launch gets its own slot and its weight-norm chain rule is queued;
+    `flush()` runs all queued jobs in ONE nero_wgrad_finish_batch launch.
     Jobs that would accumulate into the same gradient rows are never queued together (the queue is flushed first), so the
     batched kernel has no write conflicts."""
 
     def __init__(self, device, P=66, rows=256, ld=384, max_slots=48):
         self.P, self.rows, self.ld = P, rows, ld
         self.device, self.max_slots = device, max_slots
-        # slot i = acc[i] [P, rows, ld] followed by its bias sums [P, rows]; zero = ready to accumulate into.  Slots are made
-        # on first use and kept, so their addresses stay valid for graph replay
+        # slot i = slices[i] [P, rows, ld] followed by its bias sums [P, rows].  Slots are made on first use and kept, so their
+        # addresses stay valid for graph replay
         self.slots = []
         self.jobs, self.dest, self.keep = [], set(), []
         self.defer = False
@@ -288,7 +289,7 @@ class WgradWorkspace:
     def _slot(self):
         i = len(self.jobs)
         while len(self.slots) <= i:
-            self.slots.append(torch.zeros(self.P * (self.rows * self.ld + self.rows), dtype=torch.float32, device=self.device))
+            self.slots.append(torch.empty(self.P * (self.rows * self.ld + self.rows), dtype=torch.float32, device=self.device))
         row = self.slots[i]
         n = self.P * self.rows * self.ld
         return row[:n].view(self.P, self.rows, self.ld), row[n:].view(self.P, self.rows)
@@ -323,7 +324,6 @@ class WgradWorkspace:
                                      int(arr['K'].max()))
         tab, max_rows, max_k = hit
         K('nero_wgrad_finish_batch', tab, len(self.jobs), max_rows, max_k)
-        torch._foreach_zero_(self.slots[:len(self.jobs)])     # the used accumulators are ready for the next pass
         self.jobs, self.dest, self.keep = [], set(), []
 
 
@@ -335,14 +335,12 @@ def wgrad(ws: WgradWorkspace, dY: Mat, n_valid, X: Mat, k_valid, layer: Prepared
         m_cap = dY.t.shape[0]
     n_rows_pad = ceil_div(n_valid, 16) * 16
     k_pad = ceil_div(layer.k_layout, 64) * 64
-    assert k_pad <= ws.ld and n_rows_pad <= ws.rows
+    # the finish reads slice rows [0, nrows) and columns kmap[k] < k_layout: all inside the window the launches store
+    assert k_pad <= ws.ld and n_rows_pad <= ws.rows and layer.nrows <= n_rows_pad
     if ws.defer and grad_w is not None and (grad_w.data_ptr(), layer.row0) in ws.dest:
         ws.flush()                      # a queued job already accumulates into these rows
     partial_t, bias_t = ws.partial, ws.bias_partial
-    P = ws.P          # row slices per 128-row output tile, one accumulator slice each
-    if not ws.defer:          # stand-alone use: the accumulator slot is zeroed per call
-        partial_t.zero_()
-        bias_t.zero_()
+    P = ws.P          # row slices per 128-row output tile, one slice each
     K('nero_wgrad', dY, dY.ld, n_valid, X, X.ld, k_valid, dY2, dY2.ld if dY2 else 0, X2, X2.ld if X2 else 0,
       partial_t, ws.ld, ws.rows, bias_t, n_rows_pad, k_pad, P, m_ptr, m_cap,
       launches=ceil_div(n_rows_pad, 128) * max(1, ceil_div(k_pad, 256)))
