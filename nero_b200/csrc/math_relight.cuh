@@ -7,6 +7,7 @@
 #include <cstdint>
 
 #include "common.cuh"
+#include "hash.cuh"
 #include "math_mc.cuh"
 
 namespace nero {
@@ -14,12 +15,6 @@ namespace nero {
 constexpr float kRelightEps = 1e-4f;      // offset of spawned rays along the side normal
 constexpr float kRelightMinAlpha = 1e-3f; // GGX sampling floor of alpha (the BRDF itself uses the unclamped alpha)
 
-NERO_HD uint32_t rl_mix(uint32_t x) {     // murmur3 finaliser
-  x ^= x >> 16; x *= 0x85ebca6bu;
-  x ^= x >> 13; x *= 0xc2b2ae35u;
-  x ^= x >> 16;
-  return x;
-}
 // uniform in [0, 1) with 24 random bits, a pure function of (seed, pixel, sample, bounce, dim)
 NERO_HD float rl_uniform(uint32_t seed, uint32_t pixel, uint32_t sample, uint32_t bounce, uint32_t dim) {
   uint32_t h = rl_mix(seed * 0x9e3779b9u + 0x7f4a7c15u);

@@ -31,6 +31,23 @@ Three consequences of the reference's rasteriser call, reproduced on purpose:
 
 Two boundaries are restated rather than pinned (DESIGN.md section 2): nvdiffrast's coverage rule on silhouette edges (a ray
 cast counts a pixel centre on an edge as covered) and Open3D's output order (hash order; here ascending voxel key).
+
+The real-data protocol (the reference's eval.md, "Evaluate the Glossy Real dataset") cleans the stage-I mesh by hand in
+MeshLab, samples 500 k points uniformly on its surface and on the ground-truth mesh in CloudCompare, and runs
+eval_real_shape.py on the two clouds.  clean_mesh and sample_surface replace the two GUI steps (k_meshpts.cu):
+  * Crop.  A triangle is kept iff its three vertices lie inside the sphere (centre, radius) and / or the axis-aligned box,
+    tested in fp64.  Triangles are never clipped.
+  * Components.  Two kept triangles are connected when they share a vertex index (vertices are not welded by position:
+    marching cubes shares them exactly).  A component's label is its smallest vertex index.
+  * Selection.  A component's area is the fp64 sum of its triangles' areas 0.5 |(v1 - v0) x (v2 - v0)| in ascending
+    triangle index; it is kept iff its area >= min_component * the largest component's area (0 keeps everything).  The
+    kept triangles and the vertices they reference keep their original order.
+  * Sampling.  Sample i of a seed takes the first triangle whose inclusive cumulative area exceeds u0 * total area, with a
+    53-bit uniform u0, and the point (1 - s) v0 + s (1 - r2) v1 + s r2 v2 with s = sqrt(r1): i.i.d. area-uniform samples.
+    Each sample depends on (seed, i) and the mesh only, so a cloud is the same however it is split into launches.
+Two third-party boundaries are restated rather than pinned (DESIGN.md section 2): the MeshLab step is an explicit crop plus
+the area-fraction rule, not a hand selection, and no claim is made about CloudCompare's sampling scheme beyond
+area-uniformity.
 """
 import os
 import pickle
@@ -220,6 +237,156 @@ def chamfer_distance(pts_gt, pts_pr):
 def result_line(stem, chamfer):
     """The line the reference prints and appends to data/geometry.log."""
     return f'{stem} {chamfer:.5f}'
+
+
+# ------------------------------------------------------------------------------------------------ mesh clean-up and sampling
+_BLOCK = 256                  # NERO_MESHPTS_BLOCK / NERO_MESHPTS_CHUNK (include/nero_meshpts.h)
+_INT32_MAX = 2 ** 31 - 1
+
+
+def _check_mesh_shape(v_shape, t_shape, what):
+    if len(v_shape) != 2 or v_shape[1] != 3 or len(t_shape) != 2 or t_shape[1] != 3:
+        raise ValueError(f'{what} needs verts [V,3] and tris [T,3], got {tuple(v_shape)} and {tuple(t_shape)}')
+    if v_shape[0] < 1 or t_shape[0] < 1:
+        raise ValueError(f'{what}: the mesh is empty ({v_shape[0]} vertices, {t_shape[0]} triangles)')
+    if v_shape[0] > _INT32_MAX or t_shape[0] > _INT32_MAX:
+        raise ValueError(f'{what}: {v_shape[0]} vertices / {t_shape[0]} triangles do not fit int32 indices')
+
+
+def _mesh_cuda(verts, tris, what):
+    """(verts float32 [V,3], tris int32 [T,3]) as contiguous CUDA tensors from numpy arrays or tensors.  The shapes, the index
+    range and finiteness are checked (on the host for numpy input) before any kernel runs."""
+    torch = _torch()
+    if torch.is_tensor(verts) or torch.is_tensor(tris):
+        v, t = torch.as_tensor(verts).detach(), torch.as_tensor(tris).detach()
+        _check_mesh_shape(v.shape, t.shape, what)
+        dev = v.device if v.device.type == 'cuda' else t.device if t.device.type == 'cuda' else torch.device('cuda')
+        v = v.to(dev, torch.float32).contiguous()
+        t = t.to(dev, torch.int64)
+        lo, hi = int(t.min()), int(t.max())
+        finite = bool(torch.isfinite(v).all())
+        t = t.to(torch.int32).contiguous()
+    else:
+        v, t = np.asarray(verts), np.asarray(tris)
+        _check_mesh_shape(v.shape, t.shape, what)
+        if not np.issubdtype(t.dtype, np.integer):
+            raise ValueError(f'{what}: triangle indices must be integers, got {t.dtype}')
+        lo, hi = int(t.min()), int(t.max())
+        v = np.ascontiguousarray(v, np.float32)
+        finite = bool(np.isfinite(v).all())
+    if lo < 0 or hi >= v.shape[0]:
+        raise ValueError(f'{what}: triangle index out of range [0, {v.shape[0]}): min {lo}, max {hi}')
+    if not finite:
+        raise ValueError(f'{what}: vertex coordinates must be finite')
+    if not torch.is_tensor(v):
+        v = torch.from_numpy(v).cuda()
+        t = torch.from_numpy(np.ascontiguousarray(t, np.int32)).cuda()
+    _ops().require_cuda(v.device, what)
+    return v, t
+
+
+def _region(sphere, box, min_component):
+    """Host copies of the crop arguments (None or float64 arrays), checked."""
+    if not 0.0 <= min_component <= 1.0:
+        raise ValueError(f'min_component must lie in [0, 1], got {min_component}')
+    sph = bx = None
+    if sphere is not None:
+        sph = np.ascontiguousarray(sphere, np.float64).reshape(-1)
+        if sph.shape != (4,) or not np.isfinite(sph).all():
+            raise ValueError(f'sphere must be 4 finite numbers (cx, cy, cz, r), got {sphere}')
+        if not sph[3] > 0:
+            raise ValueError(f'sphere radius must be positive, got {sph[3]}')
+    if box is not None:
+        bx = np.ascontiguousarray(box, np.float64).reshape(-1)
+        if bx.shape != (6,) or not np.isfinite(bx).all():
+            raise ValueError(f'box must be 6 finite numbers (x0, y0, z0, x1, y1, z1), got {box}')
+        if not (bx[:3] <= bx[3:]).all():
+            raise ValueError(f'box needs x0 <= x1, y0 <= y1, z0 <= z1, got {box}')
+    return sph, bx
+
+
+def clean_mesh_cuda(verts, tris, sphere=None, box=None, min_component=0.0):
+    """clean_mesh with its intermediate results: (verts, tris, info).  info holds CUDA tensors area [T] (fp64), keep [T]
+    (uint8, the crop), label [T] (int32; V for cropped triangles), comp_label [m] (int32, ascending), comp_area [m] (fp64),
+    comp_keep [m] (bool), and the ints triangles, components, kept_components, kept_triangles, kept_vertices."""
+    torch = _torch()
+    ops = _ops()
+    sph, bx = _region(sphere, box, min_component)
+    v, t = _mesh_cuda(verts, tris, 'clean_mesh')
+    V, T = v.shape[0], t.shape[0]
+    dev = v.device
+    with torch.cuda.device(dev):
+        area = torch.empty(T, dtype=torch.float64, device=dev)
+        keep = torch.empty(T, dtype=torch.uint8, device=dev)
+        ops.K('nero_meshpts_areas', v, V, t, T, sph, bx, area, keep)
+        parent = torch.empty(V, dtype=torch.int32, device=dev)
+        label = torch.empty(T, dtype=torch.int32, device=dev)
+        ops.K('nero_meshpts_components', t, T, keep, V, parent, label, launches=4 + (V - 1).bit_length())
+        skeys, order = torch.sort(label, stable=True)    # plumbing: stable, so each component lists its triangles in order
+        labs, counts = torch.unique_consecutive(skeys, return_counts=True)
+        ends = torch.cumsum(counts, 0)
+        if int(labs[-1]) == V:                           # the cropped triangles
+            labs, ends = labs[:-1], ends[:-1]
+        m = labs.shape[0]
+        if m == 0:
+            raise ValueError('clean_mesh: no triangle lies inside the crop region')
+        comp_area = torch.empty(m, dtype=torch.float64, device=dev)
+        root_keep = torch.empty(V, dtype=torch.uint8, device=dev)
+        ops.K('nero_meshpts_component_areas', area, order, ends, labs, m, float(min_component), comp_area, root_keep, launches=2)
+        nbt, nbv = ops.ceil_div(T, _BLOCK), ops.ceil_div(V, _BLOCK)
+        tri_flag = torch.empty(T, dtype=torch.uint8, device=dev)
+        vert_flag = torch.empty(V, dtype=torch.uint8, device=dev)
+        blk_cnt = torch.empty(nbt + nbv, dtype=torch.int32, device=dev)
+        blk_off = torch.empty(nbt + nbv, dtype=torch.int64, device=dev)
+        totals = torch.empty(2, dtype=torch.int64, device=dev)
+        ops.K('nero_meshpts_compact_count', t, T, keep, label, root_keep, V, tri_flag, vert_flag, blk_cnt, blk_off, totals, launches=5)
+        nv, nt = totals.tolist()
+        remap = torch.empty(V, dtype=torch.int32, device=dev)
+        vo = torch.empty(nv, 3, dtype=torch.float32, device=dev)
+        to = torch.empty(nt, 3, dtype=torch.int32, device=dev)
+        ops.K('nero_meshpts_compact_emit', v, V, t, T, tri_flag, vert_flag, blk_off, nv, nt, remap, vo, to, launches=2)
+        comp_keep = root_keep[labs.long()].bool()
+    info = dict(area=area, keep=keep, label=label, comp_label=labs, comp_area=comp_area, comp_keep=comp_keep, triangles=T,
+                components=m, kept_components=int(comp_keep.sum()), kept_triangles=nt, kept_vertices=nv)
+    return vo, to, info
+
+
+def clean_mesh(verts, tris, sphere=None, box=None, min_component=0.0):
+    """Replaces the MeshLab step of the real-data protocol: crop to the sphere (cx, cy, cz, r) and / or the box (x0, y0, z0,
+    x1, y1, z1), split the rest into connected components and keep those whose area is at least min_component (in [0, 1])
+    times the largest one's.  verts [V,3] / tris [T,3] as numpy arrays or tensors -> (verts CUDA float32 [V',3], tris CUDA
+    int32 [T',3]): the kept triangles and the vertices they use, in their original order."""
+    v, t, _ = clean_mesh_cuda(verts, tris, sphere, box, min_component)
+    return v, t
+
+
+def sample_surface(verts, tris, n, seed=0, first=0):
+    """Replaces CloudCompare's 'sample points on a mesh': n i.i.d. area-uniform points on the surface -> CUDA float64 [n,3].
+    Returns samples first .. first + n - 1 of the seed's sequence, so a cloud can be produced in pieces.  Raises ValueError
+    for an empty mesh or one without area."""
+    torch = _torch()
+    ops = _ops()
+    if int(n) != n or n < 1:
+        raise ValueError(f'sample_surface needs n >= 1 points, got {n}')
+    if int(seed) != seed or not 0 <= seed < 2 ** 32:
+        raise ValueError(f'seed must be an integer in [0, 2^32), got {seed}')
+    if int(first) != first or first < 0:
+        raise ValueError(f'first must be a non-negative integer, got {first}')
+    v, t = _mesh_cuda(verts, tris, 'sample_surface')
+    V, T = v.shape[0], t.shape[0]
+    dev = v.device
+    with torch.cuda.device(dev):
+        area = torch.empty(T, dtype=torch.float64, device=dev)
+        ops.K('nero_meshpts_areas', v, V, t, T, None, None, area, None)
+        chunk = torch.empty(ops.ceil_div(T, _BLOCK), dtype=torch.float64, device=dev)
+        cdf = torch.empty(T, dtype=torch.float64, device=dev)
+        ops.K('nero_meshpts_cdf', area, T, chunk, cdf, launches=3)
+        total = float(cdf[-1])
+        if not (total > 0 and np.isfinite(total)):
+            raise ValueError(f'sample_surface: the mesh has no surface area (total {total})')
+        out = torch.empty(int(n), 3, dtype=torch.float64, device=dev)
+        ops.K('nero_meshpts_sample', v, V, t, T, cdf, int(seed), int(first), int(n), out)
+    return out
 
 
 # ------------------------------------------------------------------------------------------------ GlossySynthetic data
