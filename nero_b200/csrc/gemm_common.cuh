@@ -58,16 +58,18 @@ __device__ __forceinline__ void mma_split3(float* d, uint64_t a_hi, uint64_t a_l
 // two adjacent fp32 values (col, col + 1) (col even) of one row; columns >= lim and rows that are not ok read as zero.
 // g is 8-byte aligned and ld even (checked at launch), so at an even lim every pair is one 8-byte load; at an odd lim
 // the last pair has one column and every pair takes two 4-byte loads.  The loads are predicated rather than branched
-// around, so a caller can issue many of them before it uses the first.
+// around, so a caller can issue many of them before it uses the first.  Each epilogue operand is read once per launch, so
+// the loads are streaming (ld.global.cs: evict-first in L1 and L2) and leave L2 to the weight images every CTA re-reads;
+// with the default policy the gradient sweeps ran about 1.5x longer on an H100 (DESIGN.md section 6).
 template <bool kEvenLim>
 __device__ __forceinline__ float2 ld2(const float* __restrict__ g, int ld, long row, int col, int lim, bool ok) {
   const float* q = g + row * ld + col;
   float2 x = make_float2(0.f, 0.f);
   if constexpr (kEvenLim) {
-    if (ok && col < lim) x = __ldg(reinterpret_cast<const float2*>(q));
+    if (ok && col < lim) x = __ldcs(reinterpret_cast<const float2*>(q));
   } else {
-    if (ok && col < lim) x.x = __ldg(q);
-    if (ok && col + 1 < lim) x.y = __ldg(q + 1);
+    if (ok && col < lim) x.x = __ldcs(q);
+    if (ok && col + 1 < lim) x.y = __ldcs(q + 1);
   }
   return x;
 }
