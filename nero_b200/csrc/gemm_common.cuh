@@ -55,6 +55,17 @@ __device__ __forceinline__ void mma_split3(float* d, uint64_t a_hi, uint64_t a_l
   Wgmma<N>::template mma<TA, TB>(d, a_hi, b_hi, 1);
 }
 
+// L2 policy of the GEMM kernels: every CTA re-reads each layer's weight image from L2, while a launch streams hundreds of
+// MB of row operands and results that it touches once.  The weight copies are evict-last, and the row operands (first A
+// operand, the chain's skip-concat source, epilogue operands) and the results are read and written with streaming
+// accesses (ld / st.global.cs: evict-first), so that stream does not push the weights out of L2.  Bias vectors, which
+// every CTA re-reads, keep the default policy.  On an H100 the evict-last copies alone measured no faster, but on top of
+// the streaming accesses they take another ~1.8 ms off the chain launches of a step (DESIGN.md section 6).
+__device__ __forceinline__ void weight_copy(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
+  bulk_copy_g2s(smem_dst, gmem_src, bytes, bar, l2_policy_evict_last());
+}
+__device__ __forceinline__ float4 ld_stream4(const float* g) { return __ldcs(reinterpret_cast<const float4*>(g)); }
+
 // two adjacent fp32 values (col, col + 1) (col even) of one row; columns >= lim and rows that are not ok read as zero.
 // g is 8-byte aligned and ld even (checked at launch), so at an even lim every pair is one 8-byte load; at an odd lim
 // the last pair has one column and every pair takes two 4-byte loads.  The loads are predicated rather than branched
@@ -80,9 +91,9 @@ inline bool pair_aligned(const float* g, int ld) {
 __device__ __forceinline__ void st2(float* __restrict__ g, int ld, long row, int col, int lim, bool ok, float a, float b) {
   if (!ok || !g || col >= lim) return;
   float* q = g + row * ld + col;
-  if (col + 1 < lim && (reinterpret_cast<uintptr_t>(q) & 7) == 0) { *reinterpret_cast<float2*>(q) = make_float2(a, b); return; }
-  q[0] = a;
-  if (col + 1 < lim) q[1] = b;
+  if (col + 1 < lim && (reinterpret_cast<uintptr_t>(q) & 7) == 0) { __stcs(reinterpret_cast<float2*>(q), make_float2(a, b)); return; }
+  __stcs(q, a);
+  if (col + 1 < lim) __stcs(q + 1, b);
 }
 
 // operands of the epilogue of one layer (nero_linear / one layer of nero_chain; see include/nero_b200.h)
@@ -151,8 +162,8 @@ __device__ __forceinline__ float2 epi_pair(const EpiArgs& e, long row, int col, 
     }
     // skip-branch columns [ncol_main, ncol_out) carry oscale * acc and go to the tail buffer
     if (e.tail && row_ok) {
-      if (col >= e.ncol_main && col < e.ncol_out) e.tail[row * e.ldt + (col - e.ncol_main)] = e.oscale * v0;
-      if (col + 1 >= e.ncol_main && col + 1 < e.ncol_out) e.tail[row * e.ldt + (col + 1 - e.ncol_main)] = e.oscale * v1;
+      if (col >= e.ncol_main && col < e.ncol_out) __stcs(e.tail + row * e.ldt + (col - e.ncol_main), e.oscale * v0);
+      if (col + 1 >= e.ncol_main && col + 1 < e.ncol_out) __stcs(e.tail + row * e.ldt + (col + 1 - e.ncol_main), e.oscale * v1);
     }
   }
   st2(e.out, e.ldo, row, col, nmain, row_ok, r0, r1);

@@ -46,7 +46,7 @@ __device__ __forceinline__ void put_a2(uint8_t* s_a, int r, int col, float y0, f
   sts_u32(q + kAPlane, lo);
 }
 __device__ __forceinline__ float csrc_at(const nero_chain_layer& L, long row, int col, bool row_ok) {
-  return (L.csrc && row_ok) ? __ldg(L.csrc + row * L.ld_csrc + col) : 0.0f;
+  return (L.csrc && row_ok) ? __ldcs(L.csrc + row * L.ld_csrc + col) : 0.0f;
 }
 
 // position of the next weight stage to load in the (tile, layer, N half, K chunk) sequence the MMAs walk
@@ -75,8 +75,8 @@ __device__ __forceinline__ void w_issue(const nero_chain_params& p, ConsumerCtx&
   const uint32_t bytes = min(kHalfBytes, plane - q.hf * kHalfBytes);
   const uint8_t* src = static_cast<const uint8_t*>(L.wimg) + size_t(q.kc) * 2u * plane + size_t(q.hf) * kHalfBytes;
   mbar_arrive_expect_tx(&c.full[s], 2u * bytes);
-  bulk_copy_g2s(c.s_w + s * kWStageBytes, src, bytes, &c.full[s]);
-  bulk_copy_g2s(c.s_w + s * kWStageBytes + kHalfBytes, src + plane, bytes, &c.full[s]);
+  weight_copy(c.s_w + s * kWStageBytes, src, bytes, &c.full[s]);
+  weight_copy(c.s_w + s * kWStageBytes + kHalfBytes, src + plane, bytes, &c.full[s]);
   ++q.g;
   if (++q.kc == L.k_chunks) {
     q.kc = 0;
@@ -194,7 +194,7 @@ __global__ void __launch_bounds__(kChThreads, 1) gemm_chain_kernel(const __grid_
           const int i = lane + 32 * (4 * b + u), rl = c.wg * 64 + c.w * 16 + i / n4, col = 4 * (i % n4);
           const float* q = p.A0 + (long(tile) * CH_BM + rl) * p.lda0 + col;    // 16-byte aligned: checked at launch
           x[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (rl < rows_valid && col < p.k_valid0) x[u] = __ldg(reinterpret_cast<const float4*>(q));
+          if (rl < rows_valid && col < p.k_valid0) x[u] = ld_stream4(q);
         }
 #pragma unroll
         for (int u = 0; u < 4; ++u) {

@@ -77,14 +77,14 @@ __global__ void __launch_bounds__(kLinearThreads, 1) gemm_linear_kernel(const Li
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         const int r = tile * BM + lr + 16 * i;
-        x[i] = (kcol < p.k_valid && r < M) ? __ldg(reinterpret_cast<const float4*>(p.A + size_t(r) * p.lda + kcol))
+        x[i] = (kcol < p.k_valid && r < M) ? ld_stream4(p.A + size_t(r) * p.lda + kcol)
                                             : make_float4(0.f, 0.f, 0.f, 0.f);
       }
       // every warpgroup has finished the MMAs of chunk g - 2 (wgmma_wait<1> below): stage s is free
       __syncthreads();
       if (tid == 0) {
         mbar_arrive_expect_tx(&full[s], 2 * Cfg::b_plane);
-        bulk_copy_g2s(st + 2 * kABytes, p.wimg + size_t(c) * 2 * Cfg::b_plane, 2 * Cfg::b_plane, &full[s]);
+        weight_copy(st + 2 * kABytes, p.wimg + size_t(c) * 2 * Cfg::b_plane, 2 * Cfg::b_plane, &full[s]);
       }
 #pragma unroll
       for (int i = 0; i < 8; ++i) {

@@ -61,11 +61,21 @@ __device__ __forceinline__ void named_bar(int id, int count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
+// ------------------------------------------------------------------ L2 cache policies (per-instruction hints)
+// lines an access with this policy brings into L2 are evicted after normal and evict-first lines
+__device__ __forceinline__ uint64_t l2_policy_evict_last() {
+  uint64_t pol;
+  asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+  return pol;
+}
+
 // ------------------------------------------------------------------ bulk async copy global -> shared (UBLKCP)
-__device__ __forceinline__ void bulk_copy_g2s(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
+// with the L2 policy `l2_policy` (createpolicy) for the source lines
+__device__ __forceinline__ void bulk_copy_g2s(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar, uint64_t l2_policy) {
   asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(smem_dst)),
-      "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
+          smem_u32(smem_dst)),
+      "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)), "l"(l2_policy)
       : "memory");
 }
 
