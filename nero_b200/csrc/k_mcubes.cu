@@ -12,12 +12,11 @@
 // atomics decide where anything goes, so the output is bit-identical run to run.  The triangle pass finds the vertex ids of
 // its cube's edges in `emap` (edge key 3*L + a -> vertex id), which the vertex pass fills at sign-change edges only.
 #include "common.cuh"
-#include "mc_tables.cuh"
+#include "mc_common.cuh"
 
 namespace nero {
 namespace {
 
-constexpr int kMcbThreads = 256;
 constexpr int kMcbSub = 4;
 constexpr int kMcbTile = kMcbThreads * kMcbSub;   // keep in step with include/nero_b200.h (nblk)
 constexpr int kMcbScanThreads = 1024;
@@ -53,33 +52,8 @@ __device__ __forceinline__ void mcb_classify(const McGrid& g, long long L, int& 
     c[5] = __ldg(p + g.sx + 1);
     c[6] = __ldg(p + g.nz + 1);
     c[7] = __ldg(p + g.sx + g.nz + 1);
-    cs = 0;
-#pragma unroll
-    for (int q = 0; q < 8; ++q) cs |= (c[q] <= iso ? 1 : 0) << q;
+    cs = mc_case(c, iso);
   }
-}
-
-// exclusive prefix of x over the block in thread order; *total = block sum.  s_w: kMcbThreads/32 ints.
-__device__ __forceinline__ int mcb_block_scan(int x, int* s_w, int* total) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  int incl = x;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int v = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += v;
-  }
-  if (lane == 31) s_w[wid] = incl;
-  __syncthreads();
-  int before = 0, tot = 0;
-#pragma unroll
-  for (int w = 0; w < kMcbThreads / 32; ++w) {
-    const int v = s_w[w];
-    before += w < wid ? v : 0;
-    tot += v;
-  }
-  __syncthreads();
-  *total = tot;
-  return before + incl - x;
 }
 
 __global__ void __launch_bounds__(kMcbThreads) mcubes_count_kernel(const McGrid g, int* __restrict__ blk_cnt) {
@@ -113,15 +87,6 @@ __global__ void __launch_bounds__(kMcbThreads) mcubes_count_kernel(const McGrid 
     blk_cnt[2 * blockIdx.x] = a;
     blk_cnt[2 * blockIdx.x + 1] = b;
   }
-}
-
-__device__ __forceinline__ long long mcb_warp_incl(long long x, int lane) {
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const long long v = __shfl_up_sync(0xffffffffu, x, o);
-    if (lane >= o) x += v;
-  }
-  return x;
 }
 
 // one block: exclusive scan of the (vertex, triangle) block counts in block order, and the two totals
@@ -170,8 +135,7 @@ __global__ void __launch_bounds__(kMcbThreads) mcubes_verts_kernel(const McGrid 
 #pragma unroll
     for (int a = 0; a < 3; ++a) {
       if (em >> a & 1) {
-        const float far = c[1 << a];
-        const float t = (g.iso - c[0]) / (far - c[0]);
+        const float t = mc_interp(g.iso, c[0], c[1 << a]);
         float* row = s_v + 3 * off;
         row[0] = float(i) + (a == 0 ? t : 0.f);
         row[1] = float(j) + (a == 1 ? t : 0.f);

@@ -403,6 +403,28 @@ class NeROShapeRenderer(nn.Module):
         vertices = v.cpu().numpy().astype(np.float64) / (resolution - 1.0) * (bmax - bmin)[None, :] + bmin[None, :]
         return vertices, t.cpu().numpy().astype(np.int64)
 
+    def extract_mesh_sparse(self, resolution=1024, threshold=0.0, bound_min=-1.0, bound_max=1.0, brick=8, lipschitz=2.0,
+                            return_stats=False):
+        """extract_mesh without the dense grid: the SDF is sampled in a narrow band of brick^3-cube bricks around the surface
+        only (nero_b200.mesh.extract_sparse, k_mcsparse.cu), so the cost follows the surface area and 1024^3 or 2048^3 grids
+        fit one card.  Same grid points, same SDF values and same unit-sphere override as extract_mesh, so the arrays equal
+        extract_mesh's bit for bit, with one limit: a closed piece of surface smaller than a brick, lying between brick
+        corners where the SDF is steeper than `lipschitz`, is not found (raise `lipschitz` or lower `brick`).  Returns what
+        extract_mesh returns, and extract_sparse's statistics too with return_stats."""
+        from .mesh import extract_sparse
+        bmin = np.broadcast_to(np.asarray(bound_min, np.float32), (3,))
+        bmax = np.broadcast_to(np.asarray(bound_max, np.float32), (3,))
+        dev = self.deviation_network.variance.device
+        axes = [torch.linspace(float(bmin[i]), float(bmax[i]), resolution, device=dev) for i in range(3)]
+
+        def query(pts):
+            with torch.no_grad():
+                return self.engine.sdf_query(pts)[:, 0]
+        v, t, stats = extract_sparse(query, axes, threshold, brick=brick, lipschitz=lipschitz, outside=1.0)
+        vertices = v.cpu().numpy().astype(np.float64) / (resolution - 1.0) * (bmax - bmin)[None, :] + bmin[None, :]
+        triangles = t.cpu().numpy().astype(np.int64)
+        return (vertices, triangles, stats) if return_stats else (vertices, triangles)
+
     def extract_geometry(self, bound_min=(-1.0, -1.0, -1.0), bound_max=(1.0, 1.0, 1.0), resolution=128, threshold=0.0):
         """extract_geometry (network/field.py:1106-1113): marching cubes on the field; the cubes stay third party (PyMCubes,
         as in the reference) and are imported here, where they are needed."""

@@ -1,10 +1,15 @@
 """Stage-I checkpoint -> triangle mesh for stage II, on the GPU (the reference's extract_mesh.py).
 
-    python tools/extract_mesh.py --cfg configs/shape/syn/bell.yaml [--resolution 512]
+    python tools/extract_mesh.py --cfg configs/shape/syn/bell.yaml [--resolution 512] [--sparse [--brick 8] [--lipschitz 2.0]]
 
 Loads data/model/<name>/model.pth ({'step', 'network_state_dict', ...}), samples the SDF on a resolution^3 grid over [-1,1]^3
 (1.0 outside the unit sphere), runs marching cubes at level 0 and writes data/meshes/<name>-<step>.ply, the path
 NeROMaterialRenderer's `mesh` option and predict_materials read.  Paths are relative to the working directory.
+
+With --sparse the SDF is sampled only in bricks of brick^3 cubes around the surface (NeROShapeRenderer.extract_mesh_sparse):
+the same mesh, at a cost that follows the surface, which is what makes --resolution 1024 and 2048 possible on one card.  A
+closed piece of surface smaller than a brick where the SDF is steeper than --lipschitz can be missed; raise --lipschitz or
+lower --brick then.
 """
 import argparse
 import os
@@ -19,6 +24,9 @@ def main(argv=None):
     parser = argparse.ArgumentParser(description=__doc__.split('\n')[0])
     parser.add_argument('--cfg', type=str, required=True)
     parser.add_argument('--resolution', type=int, default=512)
+    parser.add_argument('--sparse', action='store_true', help='sample the SDF in a narrow band around the surface only')
+    parser.add_argument('--brick', type=int, default=8, choices=(4, 8, 16), help='cubes per brick edge (with --sparse)')
+    parser.add_argument('--lipschitz', type=float, default=2.0, help='bound on the SDF slope used for seeding (with --sparse)')
     flags = parser.parse_args(argv)
 
     import torch
@@ -37,11 +45,18 @@ def main(argv=None):
     network = network.eval().cuda()
     print(f'successfully load {cfg["name"]} step {step}!')
 
-    vertices, triangles = network.extract_mesh(resolution=flags.resolution, threshold=0.0)
+    stats = None
+    if flags.sparse:
+        vertices, triangles, stats = network.extract_mesh_sparse(resolution=flags.resolution, threshold=0.0, brick=flags.brick,
+                                                                 lipschitz=flags.lipschitz, return_stats=True)
+    else:
+        vertices, triangles = network.extract_mesh(resolution=flags.resolution, threshold=0.0)
     os.makedirs('data/meshes', exist_ok=True)
     path = os.path.join('data', 'meshes', f'{cfg["name"]}-{step}.ply')
     write_ply(path, vertices, triangles)
     print(f'{path}: {vertices.shape[0]} vertices, {triangles.shape[0]} triangles')
+    if stats is not None:
+        print('sparse: ' + ', '.join(f'{k} {v}' for k, v in stats.items()))
     return path
 
 
