@@ -90,7 +90,7 @@ def _read(f, fmt):
     return struct.unpack(fmt, b)
 
 
-def _read_bin(path):
+def _read_bin(path, tracks=None):
     cameras, images, pts = {}, {}, []
     with open(os.path.join(path, 'cameras.bin'), 'rb') as f:
         for _ in range(_read(f, '<Q')[0]):
@@ -114,7 +114,10 @@ def _read_bin(path):
         for _ in range(_read(f, '<Q')[0]):
             rec = _read(f, '<Q3d3BdQ')
             pts.append(rec[1:4])
-            f.seek(8 * rec[-1], 1)                                 # TRACK[] as (image_id, point2D_idx int32)
+            if tracks is None:
+                f.seek(8 * rec[-1], 1)                             # TRACK[] as (image_id, point2D_idx int32)
+            else:
+                tracks.append(np.asarray(_read(f, f'<{2 * rec[-1]}i')[0::2], np.int64))
     return cameras, images, pts
 
 
@@ -123,7 +126,7 @@ def _data_lines(path):
         return [ln.rstrip('\r\n') for ln in f if not ln.startswith('#')]
 
 
-def _read_txt(path):
+def _read_txt(path, tracks=None):
     cameras, images, pts = {}, {}, []
     for ln in _data_lines(os.path.join(path, 'cameras.txt')):
         e = ln.split()
@@ -142,19 +145,24 @@ def _read_txt(path):
         e = ln.split()
         if e:
             pts.append(tuple(float(v) for v in e[1:4]))
+            if tracks is not None:                                 # TRACK[] as (IMAGE_ID, POINT2D_IDX) after ERROR
+                tracks.append(np.asarray([int(v) for v in e[8::2]], np.int64))
     return cameras, images, pts
 
 
-def read_colmap_model(path):
-    """COLMAP sparse model in `path` (cameras, images, points3D as .bin, else .txt) -> (views, points).
+def read_colmap_model(path, tracks=False):
+    """COLMAP sparse model in `path` (cameras, images, points3D as .bin, else .txt) -> (views, points), or with
+    tracks=True (views, points, tracks).
 
     views = {image_id: (name, pose float32 [3,4] = [R | t] world -> camera, K float32 [3,3])} in file order, as
-    CustomDatabase._parse_colmap builds them; points = the sparse points float64 [P,3] in file order.  An image whose camera
-    model is not SIMPLE_RADIAL (distortion ignored), SIMPLE_PINHOLE or PINHOLE raises NotImplementedError."""
+    CustomDatabase._parse_colmap builds them; points = the sparse points float64 [P,3] in file order; tracks = one int64
+    array per point of the image ids of its track, in file order.  An image whose camera model is not SIMPLE_RADIAL
+    (distortion ignored), SIMPLE_PINHOLE or PINHOLE raises NotImplementedError."""
+    trk = [] if tracks else None
     if all(os.path.isfile(os.path.join(path, f'{n}.bin')) for n in ('cameras', 'images', 'points3D')):
-        cameras, images, pts = _read_bin(path)
+        cameras, images, pts = _read_bin(path, trk)
     elif all(os.path.isfile(os.path.join(path, f'{n}.txt')) for n in ('cameras', 'images', 'points3D')):
-        cameras, images, pts = _read_txt(path)
+        cameras, images, pts = _read_txt(path, trk)
     else:
         raise FileNotFoundError(f'{path}: no COLMAP model (cameras, images and points3D as .bin or .txt)')
     views = {}
@@ -163,6 +171,8 @@ def read_colmap_model(path):
             raise ValueError(f'{path}: image {iid} uses camera {cid}, which the model does not define')
         pose = np.concatenate([qvec2rotmat(q), np.asarray(t, np.float64)[:, None]], 1).astype(np.float32)
         views[iid] = (name, pose, _intrinsics(cameras[cid][0], cameras[cid][3]))
+    if tracks:
+        return views, np.asarray(pts, np.float64).reshape(-1, 3), trk
     return views, np.asarray(pts, np.float64).reshape(-1, 3)
 
 

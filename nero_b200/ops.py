@@ -23,6 +23,7 @@ _RELIGHT_TEX_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_reli
 _MESHPTS_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_meshpts.h')  # same library, plain-argument entry points
 _OBJPREP_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_objprep.h')  # same library, plain-argument entry points
 _MCSPARSE_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_mcsparse.h')  # same library, plain-argument entry points
+_MVS_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_mvs.h')  # same library, plain-argument entry points
 
 ACT_NONE, ACT_SOFTPLUS100, ACT_RELU, ACT_SIGMOID, ACT_EXPCLAMP = 0, 1, 2, 3, 4
 EPI_BIAS_ACT, EPI_MUL_DACT, EPI_TANGENT = 0, 1, 2
@@ -114,9 +115,10 @@ RELIGHT_TEX_PROTOS = _parse_header(_RELIGHT_TEX_HEADER)[1]
 MESHPTS_PROTOS = _parse_header(_MESHPTS_HEADER)[1]
 OBJPREP_PROTOS = _parse_header(_OBJPREP_HEADER)[1]
 MCSPARSE_PROTOS = _parse_header(_MCSPARSE_HEADER)[1]
+MVS_PROTOS = _parse_header(_MVS_HEADER)[1]
 for _name, _argtypes in (list(_PROTOS.items()) + list(TEXMAP_PROTOS.items()) + list(ENVMAP_PROTOS.items()) +
                          list(METRICS_PROTOS.items()) + list(RELIGHT_TEX_PROTOS.items()) + list(MESHPTS_PROTOS.items()) +
-                         list(OBJPREP_PROTOS.items()) + list(MCSPARSE_PROTOS.items())):
+                         list(OBJPREP_PROTOS.items()) + list(MCSPARSE_PROTOS.items()) + list(MVS_PROTOS.items())):
     _fn = getattr(lib, _name)
     _fn.argtypes, _fn.restype = _argtypes, ctypes.c_int
 # nero_abi_sizeof(i) is the size of ABI_RECORDS[i]; a library built from another version of the header would read the
