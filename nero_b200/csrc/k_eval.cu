@@ -5,7 +5,7 @@
 //                 reference's nvdiffrast call produces it with w = 1 (screen-space linear): sum b_i z_i^2 / sum b_i z_i,
 //                 0 on a miss or outside [near, far].
 //   depth_points  ordered compaction of the pixels with lo < depth < hi over a stack of views, unprojected at integer pixel
-//                 coordinates and moved to world space in fp64: count -> exclusive scan -> emit, as in k_mcubes.cu.
+//                 coordinates and moved to world space in fp64: count -> exclusive scan -> emit (compact.cuh).
 //   voxel_keys    Open3D's VoxelDownSample voxel index floor((p - min_bound) / voxel) in fp64, packed 21 bits per axis.
 //   voxel_mean    per voxel (segments of the key-sorted order) the mean of its points, summed in input order in fp64.
 //   nearest_dist  exact brute-force nearest distance: one thread per 4 queries, target tiles staged in shared memory,
@@ -14,6 +14,7 @@
 // Nothing here uses atomics to place or combine values, so every output is bit-identical from run to run.
 #include "bvh_traverse.cuh"
 #include "common.cuh"
+#include "compact.cuh"
 
 namespace nero {
 
@@ -56,30 +57,6 @@ __global__ void __launch_bounds__(128) depth_render_kernel(const nero_depth_para
 constexpr int kEvThreads = 256;
 constexpr int kEvSub = 4;
 constexpr int kEvTile = kEvThreads * kEvSub;   // keep in step with include/nero_b200.h (nblk)
-constexpr int kEvScanThreads = 1024;
-
-// exclusive prefix of x over the block in thread order; *total = block sum.  s_w: kEvThreads/32 ints.
-__device__ __forceinline__ int ev_block_scan(int x, int* s_w, int* total) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  int incl = x;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int v = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += v;
-  }
-  if (lane == 31) s_w[wid] = incl;
-  __syncthreads();
-  int before = 0, tot = 0;
-#pragma unroll
-  for (int w = 0; w < kEvThreads / 32; ++w) {
-    const int v = s_w[w];
-    before += w < wid ? v : 0;
-    tot += v;
-  }
-  __syncthreads();
-  *total = tot;
-  return before + incl - x;
-}
 
 __device__ __forceinline__ bool ev_keep(const float* depth, long long L, long long N, float lo, float hi) {
   if (L >= N) return false;
@@ -94,39 +71,8 @@ __global__ void __launch_bounds__(kEvThreads) points_count_kernel(const float* _
   int n = 0;
   for (int s = 0; s < kEvSub; ++s) n += ev_keep(depth, base + s * kEvThreads + threadIdx.x, N, lo, hi) ? 1 : 0;
   int total;
-  ev_block_scan(n, s_w, &total);
+  block_scan<kEvThreads>(n, s_w, &total);
   if (threadIdx.x == 0) blk_cnt[blockIdx.x] = total;
-}
-
-__device__ __forceinline__ long long ev_warp_incl(long long x, int lane) {
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const long long v = __shfl_up_sync(0xffffffffu, x, o);
-    if (lane >= o) x += v;
-  }
-  return x;
-}
-
-// one block: exclusive scan of the block counts in block order (chunks of 1024 with a 64-bit carry), and the total.
-// k_mcubes.cu scans interleaved (vertex, triangle) pairs; this one scans a single count per block.
-__global__ void __launch_bounds__(kEvScanThreads) points_scan_kernel(const int* __restrict__ blk_cnt, long long* __restrict__ blk_off,
-                                                                     long long* __restrict__ total, int nblk) {
-  __shared__ long long s_w[32];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  long long carry = 0;
-  for (int c0 = 0; c0 < nblk; c0 += kEvScanThreads) {
-    const int b = c0 + threadIdx.x;
-    const long long v = b < nblk ? blk_cnt[b] : 0;
-    const long long iv = ev_warp_incl(v, lane);
-    if (lane == 31) s_w[wid] = iv;
-    __syncthreads();
-    if (wid == 0) s_w[lane] = ev_warp_incl(s_w[lane], lane);
-    __syncthreads();
-    if (b < nblk) blk_off[b] = carry + (wid ? s_w[wid - 1] : 0) + iv - v;
-    carry += s_w[31];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) *total = carry;
 }
 
 // cams [n_views,16] fp64: camera -> world rotation (row-major 3x3), camera centre, fx, fy, cx, cy
@@ -141,7 +87,7 @@ __global__ void __launch_bounds__(kEvThreads) points_emit_kernel(const float* __
     const long long L = base + s * kEvThreads + threadIdx.x;
     const bool keep = ev_keep(depth, L, N, lo, hi);
     int total;
-    const int off = ev_block_scan(keep ? 1 : 0, s_w, &total);
+    const int off = block_scan<kEvThreads>(keep ? 1 : 0, s_w, &total);
     if (total == 0) continue;              // uniform across the block
     if (keep) {
       const long long view = L / hw, r = L - view * hw;
@@ -270,7 +216,7 @@ int nero_depth_points_count(const float* depth, int n_views, int height, int wid
   int nblk;
   if (!depth || !blk_cnt || !blk_off || !total || !ev_grid(n_views, height, width, N, nblk)) return NERO_ERR_ARG;
   points_count_kernel<<<nblk, kEvThreads, 0, st>>>(depth, N, lo, hi, blk_cnt);
-  points_scan_kernel<<<1, kEvScanThreads, 0, st>>>(blk_cnt, blk_off, total, nblk);
+  block_offsets<1>(blk_cnt, blk_off, total, nblk, st);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }

@@ -5,7 +5,7 @@
 //                  the three axis arrays.
 //   seed           one thread per brick: the Lipschitz test on its 8 coarse corners -> flag.
 //   compact        flags -> per-block counts -> one-block int64 scan -> emit in ascending order (appended to the brick list,
-//                  brick -> list entry written to `slot`, flags cleared), in the count / scan / emit style of k_mcubes.cu.
+//                  brick -> list entry written to `slot`, flags cleared), with the ordered compaction of compact.cuh.
 //   brick_points   one thread per point of a listed brick: (B+1)^3 rows per brick, the high-side apron included, clamped to
 //                  the grid (a clamped row repeats a boundary point; its value is never read as a grid point of its own).
 //   grow           one block per newly filled brick: a neighbour that is not listed is flagged when a grid edge in the
@@ -17,6 +17,7 @@
 //                  Placement comes from scans, not atomics; the caller sorts by key, which gives the order of k_mcubes.cu.
 //   lookup         edge key -> vertex id by binary search in the sorted vertex keys.
 #include "common.cuh"
+#include "compact.cuh"
 #include "mc_common.cuh"
 #include "../../include/nero_mcsparse.h"
 
@@ -25,7 +26,6 @@ namespace {
 
 constexpr int kMsTile = NERO_MCSPARSE_TILE;
 constexpr int kMsSub = kMsTile / kMcbThreads;
-constexpr int kMsScanThreads = 1024;
 constexpr int kMsMaxP = 17 * 17 * 17;
 constexpr int kMsGrowThreads = 128;
 
@@ -98,46 +98,8 @@ __global__ void __launch_bounds__(kMcbThreads) mcsparse_flag_count_kernel(const 
     c += i < n && flag[i] ? 1 : 0;
   }
   int total;
-  mcb_block_scan(c, s_w, &total);
+  block_scan<kMcbThreads>(c, s_w, &total);
   if (threadIdx.x == 0) blk_cnt[blockIdx.x] = total;
-}
-
-// one block: exclusive scans of kW interleaved count streams in block order, and their totals
-template <int kW>
-__global__ void __launch_bounds__(kMsScanThreads) mcsparse_scan_kernel(const int* __restrict__ cnt, long long* __restrict__ off,
-                                                                       long long* __restrict__ totals, long long nblk) {
-  __shared__ long long s_w[kW][32];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  long long carry[kW];
-#pragma unroll
-  for (int w = 0; w < kW; ++w) carry[w] = 0;
-  for (long long c0 = 0; c0 < nblk; c0 += kMsScanThreads) {
-    const long long b = c0 + threadIdx.x;
-    long long v[kW], iv[kW];
-#pragma unroll
-    for (int w = 0; w < kW; ++w) {
-      v[w] = b < nblk ? cnt[kW * b + w] : 0;
-      iv[w] = mcb_warp_incl(v[w], lane);
-      if (lane == 31) s_w[w][wid] = iv[w];
-    }
-    __syncthreads();
-    if (wid == 0) {
-#pragma unroll
-      for (int w = 0; w < kW; ++w) s_w[w][lane] = mcb_warp_incl(s_w[w][lane], lane);
-    }
-    __syncthreads();
-#pragma unroll
-    for (int w = 0; w < kW; ++w) {
-      const long long pre = wid ? s_w[w][wid - 1] : 0;
-      if (b < nblk) off[kW * b + w] = carry[w] + pre + iv[w] - v[w];
-      carry[w] += s_w[w][31];
-    }
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) {
-#pragma unroll
-    for (int w = 0; w < kW; ++w) totals[w] = carry[w];
-  }
 }
 
 __global__ void __launch_bounds__(kMcbThreads) mcsparse_flag_emit_kernel(unsigned char* __restrict__ flag, long long n,
@@ -150,7 +112,7 @@ __global__ void __launch_bounds__(kMcbThreads) mcsparse_flag_emit_kernel(unsigne
     const long long i = i0 + s * kMcbThreads + threadIdx.x;
     const int f = i < n && flag[i] ? 1 : 0;
     int total;
-    const int off = mcb_block_scan(f, s_w, &total);
+    const int off = block_scan<kMcbThreads>(f, s_w, &total);
     if (f) {
       list[at + off] = int(i);
       slot[i] = int(at + off);
@@ -264,7 +226,7 @@ __global__ void __launch_bounds__(kMcbThreads) mcsparse_count_kernel(const float
     x += __popc(em) + ((cs >= 0 ? s_nt[cs] : 0) << 16);
   }
   int total;
-  mcb_block_scan(x, s_w, &total);                           // at most 3 * 4913 vertices and 5 * 4096 triangles per brick
+  block_scan<kMcbThreads>(x, s_w, &total);                  // at most 3 * 4913 vertices and 5 * 4096 triangles per brick
   if (threadIdx.x == 0) {
     blk_cnt[2 * blockIdx.x] = total & 0xffff;
     blk_cnt[2 * blockIdx.x + 1] = total >> 16;
@@ -301,7 +263,7 @@ __global__ void __launch_bounds__(kMcbThreads) mcsparse_emit_kernel(const float*
     if (l < g.P) ms_classify(g, s_u, o, l, gp, em, cs, c);
     const int nt = cs >= 0 ? s_nt[cs] : 0;
     int total;
-    const int off = mcb_block_scan(__popc(em) + (nt << 16), s_w, &total);
+    const int off = block_scan<kMcbThreads>(__popc(em) + (nt << 16), s_w, &total);
     const long long L = gp[0] * sx + gp[1] * sy + gp[2];
     long long v = vbase + (off & 0xffff);
 #pragma unroll
@@ -379,7 +341,7 @@ int nero_mcsparse_compact_count(const unsigned char* flag, long long n, int* blk
   int nblk;
   if (!flag || n <= 0 || n > 0x7fffffffLL || !blk_cnt || !blk_off || !total || !ms_blocks(n, kMsTile, nblk)) return NERO_ERR_ARG;
   mcsparse_flag_count_kernel<<<nblk, kMcbThreads, 0, (cudaStream_t)stream>>>(flag, n, blk_cnt);
-  mcsparse_scan_kernel<1><<<1, kMsScanThreads, 0, (cudaStream_t)stream>>>(blk_cnt, blk_off, total, nblk);
+  block_offsets<1>(blk_cnt, blk_off, total, nblk, (cudaStream_t)stream);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
@@ -420,7 +382,7 @@ int nero_mcsparse_count(const float* pool, const int* list, long long n_bricks, 
   if (!ms_grid(nx, ny, nz, brick, iso, g) || !pool || !list || !blk_cnt || !blk_off || !totals) return NERO_ERR_ARG;
   if (n_bricks <= 0 || n_bricks > 0x7fffffffLL) return NERO_ERR_ARG;
   mcsparse_count_kernel<<<int(n_bricks), kMcbThreads, 0, (cudaStream_t)stream>>>(pool, list, g, blk_cnt);
-  mcsparse_scan_kernel<2><<<1, kMsScanThreads, 0, (cudaStream_t)stream>>>(blk_cnt, blk_off, totals, n_bricks);
+  block_offsets<2>(blk_cnt, blk_off, totals, n_bricks, (cudaStream_t)stream);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }

@@ -6,12 +6,13 @@
 //   vertices are ordered by (linear index of p, a), triangles by the linear index of their cube, then by table order.
 //
 // Grid points are dealt to blocks in tiles of kMcbTile consecutive linear indices.  count: per-block vertex / triangle counts;
-// scan: their exclusive scan in block order (one block walks the block totals in chunks of 1024, carrying a 64-bit running
-// sum); verts / tris: each block recomputes its counts, scans them in point order, writes its rows into shared memory and
-// copies them out as one contiguous range (a thread writing its own 12-byte rows would leave partly filled sectors).  No
-// atomics decide where anything goes, so the output is bit-identical run to run.  The triangle pass finds the vertex ids of
-// its cube's edges in `emap` (edge key 3*L + a -> vertex id), which the vertex pass fills at sign-change edges only.
+// scan: their exclusive scans in block order (compact.cuh's block_offsets over the two interleaved streams); verts / tris:
+// each block recomputes its counts, scans them in point order, writes its rows into shared memory and copies them out as one
+// contiguous range (a thread writing its own 12-byte rows would leave partly filled sectors).  No atomics decide where
+// anything goes, so the output is bit-identical run to run.  The triangle pass finds the vertex ids of its cube's edges in
+// `emap` (edge key 3*L + a -> vertex id), which the vertex pass fills at sign-change edges only.
 #include "common.cuh"
+#include "compact.cuh"
 #include "mc_common.cuh"
 
 namespace nero {
@@ -19,7 +20,6 @@ namespace {
 
 constexpr int kMcbSub = 4;
 constexpr int kMcbTile = kMcbThreads * kMcbSub;   // keep in step with include/nero_b200.h (nblk)
-constexpr int kMcbScanThreads = 1024;
 
 struct McGrid {
   const float* u;
@@ -89,35 +89,6 @@ __global__ void __launch_bounds__(kMcbThreads) mcubes_count_kernel(const McGrid 
   }
 }
 
-// one block: exclusive scan of the (vertex, triangle) block counts in block order, and the two totals
-__global__ void __launch_bounds__(kMcbScanThreads) mcubes_scan_kernel(const int* __restrict__ blk_cnt, long long* __restrict__ blk_off,
-                                                                      long long* __restrict__ totals, int nblk) {
-  __shared__ long long s_w[2][32];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  long long carry_v = 0, carry_t = 0;
-  for (int c0 = 0; c0 < nblk; c0 += kMcbScanThreads) {
-    const int b = c0 + threadIdx.x;
-    const long long v = b < nblk ? blk_cnt[2 * b] : 0, t = b < nblk ? blk_cnt[2 * b + 1] : 0;
-    const long long iv = mcb_warp_incl(v, lane), it = mcb_warp_incl(t, lane);
-    if (lane == 31) { s_w[0][wid] = iv; s_w[1][wid] = it; }
-    __syncthreads();
-    if (wid == 0) {
-      s_w[0][lane] = mcb_warp_incl(s_w[0][lane], lane);
-      s_w[1][lane] = mcb_warp_incl(s_w[1][lane], lane);
-    }
-    __syncthreads();
-    const long long pv = wid ? s_w[0][wid - 1] : 0, pt = wid ? s_w[1][wid - 1] : 0;
-    if (b < nblk) {
-      blk_off[2 * b] = carry_v + pv + iv - v;
-      blk_off[2 * b + 1] = carry_t + pt + it - t;
-    }
-    carry_v += s_w[0][31];
-    carry_t += s_w[1][31];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) { totals[0] = carry_v; totals[1] = carry_t; }
-}
-
 __global__ void __launch_bounds__(kMcbThreads) mcubes_verts_kernel(const McGrid g, const long long* __restrict__ blk_off,
                                                                    int* __restrict__ emap, float* __restrict__ verts) {
   __shared__ float s_v[3 * 3 * kMcbThreads];
@@ -130,7 +101,7 @@ __global__ void __launch_bounds__(kMcbThreads) mcubes_verts_kernel(const McGrid 
     float c[8];
     if (L < g.N) mcb_classify<false>(g, L, i, j, k, c, em, cs);
     int total;
-    int off = mcb_block_scan(__popc(em), s_w, &total);
+    int off = block_scan<kMcbThreads>(__popc(em), s_w, &total);
     if (total == 0) continue;              // uniform across the block
 #pragma unroll
     for (int a = 0; a < 3; ++a) {
@@ -176,7 +147,7 @@ __global__ void __launch_bounds__(kMcbThreads) mcubes_tris_kernel(const McGrid g
     if (L < g.N) mcb_classify<true>(g, L, i, j, k, c, em, cs);
     const int nt = cs >= 0 ? s_nt[cs] : 0;
     int total;
-    const int off = mcb_block_scan(nt, s_w, &total);
+    const int off = block_scan<kMcbThreads>(nt, s_w, &total);
     if (total == 0) continue;              // uniform across the block
     const signed char* tab = s_tri + (cs >= 0 ? cs : 0) * W;
     for (int q = 0; q < 3 * nt; ++q) s_t[3 * off + q] = emap[3 * L + s_ekey[tab[q]]];
@@ -208,7 +179,7 @@ int nero_mcubes_count(const float* u, int nx, int ny, int nz, float iso, int* bl
   int nblk;
   if (!mcb_grid(u, nx, ny, nz, iso, g, nblk) || !blk_cnt || !blk_off || !totals) return NERO_ERR_ARG;
   mcubes_count_kernel<<<nblk, kMcbThreads, 0, st>>>(g, blk_cnt);
-  mcubes_scan_kernel<<<1, kMcbScanThreads, 0, st>>>(blk_cnt, blk_off, totals, nblk);
+  block_offsets<2>(blk_cnt, blk_off, totals, nblk, st);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }

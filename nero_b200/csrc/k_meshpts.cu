@@ -1,22 +1,24 @@
 // Mesh clean-up and area-uniform surface sampling: the GPU replacement of the MeshLab clean-up and the CloudCompare sampling
 // of the real-data shape protocol.  The protocol is stated in nero_b200/evaluate.py, the ABI in include/nero_meshpts.h.
 //
-//   areas        one thread per triangle: fp64 area from the fp32 vertices (uncontracted), crop test of its three vertices.
-//   components   union-find over vertex indices: hook the larger root to the smaller by CAS (finds halve paths), then
-//                ceil(log2 V) + 1 rounds of pointer jumping, which flatten any tree of depth < V; label = root = the smallest
-//                vertex index of the component, so the result does not depend on scheduling.
+//   areas        one thread per triangle: fp64 area from the fp32 vertices (uncontracted), crop test (crop.cuh) of its three
+//                vertices.
+//   components   union-find over vertex indices (union_find.cuh): hook the larger root to the smaller by CAS (finds halve
+//                paths), then ceil(log2 V) + 1 rounds of pointer jumping, which flatten any tree of depth < V; label = root =
+//                the smallest vertex index of the component, so the result does not depend on scheduling.
 //   comp areas   one warp per component sums its triangles' areas in ascending triangle index (the order of a stable sort
 //                by label); one block takes the maximum (exact) and marks the components at or above frac * max.
-//   compaction   flags -> per-block counts -> one-block int64 scan -> emit in original order, as in k_eval.cu.
+//   compaction   flags -> per-block counts -> one-block int64 scan -> emit in original order (compact.cuh).
 //   cdf          one thread per 256-triangle chunk sums it sequentially; one thread prefixes the chunk sums; one thread per
 //                triangle adds its chunk's offset.
 //   sample       one thread per sample: counter-based hash, binary search of the cdf, barycentric point in fp64.
 //
 // Floating-point values are never combined by atomics, so every output is bit-identical from run to run.
-#include <cmath>
-
 #include "common.cuh"
+#include "compact.cuh"
+#include "crop.cuh"
 #include "hash.cuh"
+#include "union_find.cuh"
 #include "../../include/nero_meshpts.h"
 
 namespace nero {
@@ -24,24 +26,7 @@ namespace {
 
 constexpr int kBlock = NERO_MESHPTS_BLOCK;
 constexpr int kChunk = NERO_MESHPTS_CHUNK;
-constexpr int kScanThreads = 1024;
 constexpr int kSelectThreads = 1024;
-
-struct Crop {
-  int sphere, box;
-  double c[3], r2, lo[3], hi[3];
-};
-
-__device__ __forceinline__ bool inside(const Crop& q, double x, double y, double z) {
-  if (q.sphere) {
-    const double dx = __dsub_rn(x, q.c[0]), dy = __dsub_rn(y, q.c[1]), dz = __dsub_rn(z, q.c[2]);
-    if (!(__dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz)) <= q.r2)) return false;
-  }
-  if (q.box) {
-    if (!(x >= q.lo[0] && x <= q.hi[0] && y >= q.lo[1] && y <= q.hi[1] && z >= q.lo[2] && z <= q.hi[2])) return false;
-  }
-  return true;
-}
 
 __global__ void __launch_bounds__(kBlock) areas_kernel(const float* __restrict__ verts, int V, const int* __restrict__ tris, int T,
                                                        const Crop q, double* __restrict__ area, unsigned char* __restrict__ keep) {
@@ -71,37 +56,6 @@ __global__ void __launch_bounds__(kBlock) areas_kernel(const float* __restrict__
 }
 
 // ------------------------------------------------------------------------------------------------ components
-__global__ void __launch_bounds__(kBlock) uf_init_kernel(int* __restrict__ parent, int V) {
-  const int v = blockIdx.x * kBlock + threadIdx.x;
-  if (v < V) parent[v] = v;
-}
-
-// root of x with path halving.  Every parent pointer points to a smaller (or the same) index and only ever moves to an
-// ancestor, so the halving stores, racing with each other and with the hooks, keep a forest with the same roots.
-__device__ __forceinline__ int uf_find(volatile int* parent, int x) {
-  while (true) {
-    const int p = parent[x];
-    if (p == x) return x;
-    const int g = parent[p];
-    if (g != p) parent[x] = g;
-    x = g;
-  }
-}
-
-__device__ __forceinline__ void uf_unite(int* parent, int a, int b) {
-  volatile int* vp = parent;
-  while (true) {
-    a = uf_find(vp, a);
-    b = uf_find(vp, b);
-    if (a == b) return;
-    if (a > b) { const int s = a; a = b; b = s; }
-    // hook root b under the smaller root a; if b stopped being a root meanwhile, retry from its new parent
-    const int old = atomicCAS(parent + b, b, a);
-    if (old == b) return;
-    b = old;
-  }
-}
-
 __global__ void __launch_bounds__(kBlock) uf_hook_kernel(const int* __restrict__ tris, int T, const unsigned char* __restrict__ keep,
                                                          int* parent) {
   const int t = blockIdx.x * kBlock + threadIdx.x;
@@ -109,17 +63,6 @@ __global__ void __launch_bounds__(kBlock) uf_hook_kernel(const int* __restrict__
   const int i0 = __ldg(tris + 3 * (size_t)t), i1 = __ldg(tris + 3 * (size_t)t + 1), i2 = __ldg(tris + 3 * (size_t)t + 2);
   uf_unite(parent, i0, i1);
   uf_unite(parent, i0, i2);
-}
-
-// one round of pointer jumping: parent[v] <- parent[parent[v]].  Reading a value another thread has already jumped only
-// moves further up, so after k rounds parent[v] is at least the 2^k-th ancestor of v, or the root.
-__global__ void __launch_bounds__(kBlock) uf_jump_kernel(int* parent, int V) {
-  const int v = blockIdx.x * kBlock + threadIdx.x;
-  if (v >= V) return;
-  volatile int* vp = parent;
-  const int p = vp[v];
-  const int g = vp[p];
-  if (g != p) vp[v] = g;
 }
 
 __global__ void __launch_bounds__(kBlock) uf_label_kernel(const int* __restrict__ tris, int T, const unsigned char* __restrict__ keep,
@@ -180,64 +123,12 @@ __global__ void __launch_bounds__(kBlock) flag_kernel(const int* __restrict__ tr
     for (int k = 0; k < 3; ++k) vert_flag[__ldg(tris + 3 * (size_t)t + k)] = 1;   // every writer stores 1
 }
 
-// exclusive prefix of x over the block in thread order; *total = block sum.  s_w: kBlock/32 ints.
-__device__ __forceinline__ int block_scan(int x, int* s_w, int* total) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  int incl = x;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int v = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += v;
-  }
-  if (lane == 31) s_w[wid] = incl;
-  __syncthreads();
-  int before = 0, tot = 0;
-#pragma unroll
-  for (int w = 0; w < kBlock / 32; ++w) {
-    const int v = s_w[w];
-    before += w < wid ? v : 0;
-    tot += v;
-  }
-  *total = tot;
-  return before + incl - x;
-}
-
 __global__ void __launch_bounds__(kBlock) count_kernel(const unsigned char* __restrict__ flag, int n, int* __restrict__ blk_cnt) {
   __shared__ int s_w[kBlock / 32];
   const int i = blockIdx.x * kBlock + threadIdx.x;
   int total;
-  block_scan(i < n && flag[i] ? 1 : 0, s_w, &total);
+  block_scan<kBlock>(i < n && flag[i] ? 1 : 0, s_w, &total);
   if (threadIdx.x == 0) blk_cnt[blockIdx.x] = total;
-}
-
-__device__ __forceinline__ long long warp_incl(long long x, int lane) {
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const long long v = __shfl_up_sync(0xffffffffu, x, o);
-    if (lane >= o) x += v;
-  }
-  return x;
-}
-
-// one block: exclusive scan of the block counts in block order (chunks of 1024 with a 64-bit carry), and the total
-__global__ void __launch_bounds__(kScanThreads) scan_kernel(const int* __restrict__ blk_cnt, long long* __restrict__ blk_off,
-                                                            long long* __restrict__ total, int nblk) {
-  __shared__ long long s_w[32];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  long long carry = 0;
-  for (int c0 = 0; c0 < nblk; c0 += kScanThreads) {
-    const int b = c0 + threadIdx.x;
-    const long long v = b < nblk ? blk_cnt[b] : 0;
-    const long long iv = warp_incl(v, lane);
-    if (lane == 31) s_w[wid] = iv;
-    __syncthreads();
-    if (wid == 0) s_w[lane] = warp_incl(s_w[lane], lane);
-    __syncthreads();
-    if (b < nblk) blk_off[b] = carry + (wid ? s_w[wid - 1] : 0) + iv - v;
-    carry += s_w[31];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) *total = carry;
 }
 
 __global__ void __launch_bounds__(kBlock) vert_emit_kernel(const float* __restrict__ verts, int V, const unsigned char* __restrict__ flag,
@@ -247,7 +138,7 @@ __global__ void __launch_bounds__(kBlock) vert_emit_kernel(const float* __restri
   const int v = blockIdx.x * kBlock + threadIdx.x;
   const bool f = v < V && flag[v];
   int total;
-  const int r = block_scan(f ? 1 : 0, s_w, &total);
+  const int r = block_scan<kBlock>(f ? 1 : 0, s_w, &total);
   if (!f) return;
   const long long pos = blk_off[blockIdx.x] + r;
   remap[v] = int(pos);
@@ -261,7 +152,7 @@ __global__ void __launch_bounds__(kBlock) tri_emit_kernel(const int* __restrict_
   const int t = blockIdx.x * kBlock + threadIdx.x;
   const bool f = t < T && flag[t];
   int total;
-  const int r = block_scan(f ? 1 : 0, s_w, &total);
+  const int r = block_scan<kBlock>(f ? 1 : 0, s_w, &total);
   if (!f) return;
   const long long pos = blk_off[blockIdx.x] + r;
   for (int k = 0; k < 3; ++k) out[3 * pos + k] = remap[__ldg(tris + 3 * (size_t)t + k)];
@@ -348,22 +239,8 @@ extern "C" {
 int nero_meshpts_areas(const float* verts, int V, const int* tris, int T, const double* sphere, const double* box, double* area,
                        unsigned char* keep, void* stream) {
   if (!verts || !tris || !area || V < 1 || T < 1) return NERO_ERR_ARG;
-  Crop q{};
-  if (sphere) {
-    if (!(sphere[3] > 0.0) || !std::isfinite(sphere[3])) return NERO_ERR_ARG;
-    for (int a = 0; a < 3; ++a)
-      if (!std::isfinite(sphere[a])) return NERO_ERR_ARG;
-    q.sphere = 1;
-    q.c[0] = sphere[0]; q.c[1] = sphere[1]; q.c[2] = sphere[2];
-    q.r2 = sphere[3] * sphere[3];
-  }
-  if (box) {
-    for (int a = 0; a < 3; ++a)
-      if (!(box[a] <= box[3 + a])) return NERO_ERR_ARG;
-    q.box = 1;
-    for (int a = 0; a < 3; ++a) { q.lo[a] = box[a]; q.hi[a] = box[3 + a]; }
-  }
-  if ((sphere || box) && !keep) return NERO_ERR_ARG;
+  Crop q;
+  if (!make_crop(sphere, box, q) || ((sphere || box) && !keep)) return NERO_ERR_ARG;
   areas_kernel<<<nblocks(T), kBlock, 0, (cudaStream_t)stream>>>(verts, V, tris, T, q, area, keep);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
@@ -372,11 +249,9 @@ int nero_meshpts_areas(const float* verts, int V, const int* tris, int T, const 
 int nero_meshpts_components(const int* tris, int T, const unsigned char* keep, int V, int* parent, int* tri_label, void* stream) {
   if (!tris || !keep || !parent || !tri_label || V < 1 || T < 1) return NERO_ERR_ARG;
   const cudaStream_t s = (cudaStream_t)stream;
-  uf_init_kernel<<<nblocks(V), kBlock, 0, s>>>(parent, V);
+  uf_init(parent, V, s);
   uf_hook_kernel<<<nblocks(T), kBlock, 0, s>>>(tris, T, keep, parent);
-  int rounds = 1;                        // ceil(log2 V) + 1: a tree has depth < V
-  while ((1LL << (rounds - 1)) < (long long)V) ++rounds;
-  for (int r = 0; r < rounds; ++r) uf_jump_kernel<<<nblocks(V), kBlock, 0, s>>>(parent, V);
+  uf_flatten(parent, V, s);
   uf_label_kernel<<<nblocks(T), kBlock, 0, s>>>(tris, T, keep, parent, V, tri_label);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
@@ -403,8 +278,8 @@ int nero_meshpts_compact_count(const int* tris, int T, const unsigned char* keep
   flag_kernel<<<nbt, kBlock, 0, s>>>(tris, T, keep, tri_label, root_keep, tri_flag, vert_flag);
   count_kernel<<<nbt, kBlock, 0, s>>>(tri_flag, T, blk_cnt);
   count_kernel<<<nbv, kBlock, 0, s>>>(vert_flag, V, blk_cnt + nbt);
-  scan_kernel<<<1, kScanThreads, 0, s>>>(blk_cnt, blk_off, totals + 1, nbt);
-  scan_kernel<<<1, kScanThreads, 0, s>>>(blk_cnt + nbt, blk_off + nbt, totals, nbv);
+  block_offsets<1>(blk_cnt, blk_off, totals + 1, nbt, s);
+  block_offsets<1>(blk_cnt + nbt, blk_off + nbt, totals, nbv, s);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }

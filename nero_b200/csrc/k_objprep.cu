@@ -2,8 +2,8 @@
 // out of COLMAP's fused cloud, fit the support plane).  The protocol is stated in nero_b200/objprep.py, the ABI in
 // include/nero_objprep.h.
 //
-//   crop         one thread per point: the sphere / box test of k_meshpts.cu in fp64.
-//   compaction   flags -> per-block counts -> one-block int64 scan -> emit in original order, as in k_meshpts.cu.
+//   crop         one thread per point: the sphere / box test of crop.cuh in fp64.
+//   compaction   flags -> per-block counts -> one-block int64 scan -> emit in original order (compact.cuh).
 //   hypotheses   one thread per hypothesis: counter-based hash -> three kept points -> unit normal and offset in fp64.
 //   counts       the hot loop, H x n point-plane tests.  A block keeps 8 points per thread in registers and walks a tile
 //                of 256 planes staged in shared memory; each test is a warp ballot, its popcount goes to the lane that owns
@@ -12,8 +12,9 @@
 //   moments      fixed 4096-point blocks: per-thread sequential sums, a fixed shared-memory tree, then one thread per
 //                sum adds the block partials in block order, so the refit sums are bit-reproducible.
 //   above        one thread per point: height over the plane and the packed voxel key.
-//   components   union-find over the occupied voxels (sorted keys): 13 forward neighbours found by binary search, hooks
-//                to the smaller root by CAS, then ceil(log2 m) + 1 rounds of pointer jumping; label = smallest voxel index.
+//   components   union-find over the occupied voxels (sorted keys, union_find.cuh): 13 forward neighbours found by binary
+//                search, hooks to the smaller root by CAS, then ceil(log2 m) + 1 rounds of pointer jumping; label = smallest
+//                voxel index.
 //   select       integer atomics sum each component's points, one block takes the maximum and marks the kept voxels.
 //
 // Floating-point values are never combined by atomics, so every output is bit-identical from run to run.
@@ -21,7 +22,10 @@
 #include <cmath>
 
 #include "common.cuh"
+#include "compact.cuh"
+#include "crop.cuh"
 #include "hash.cuh"
+#include "union_find.cuh"
 #include "../../include/nero_objprep.h"
 
 namespace nero {
@@ -31,7 +35,6 @@ constexpr int kBlock = NERO_OBJPREP_BLOCK;
 constexpr int kChunk = NERO_OBJPREP_CHUNK;
 constexpr int kMom = NERO_OBJPREP_MOMENTS;
 constexpr int kPerThread = kChunk / kBlock;        // points per thread of a moments block
-constexpr int kScanThreads = 1024;
 constexpr int kSelectThreads = 1024;
 constexpr int kTile = 256;                         // planes per shared-memory tile of the counts
 constexpr int kPts = 8;                            // points per thread per pass of the counts
@@ -39,25 +42,9 @@ constexpr int kCountBlocks = 2048;                 // grid cap of the counts (th
 constexpr long long kVoxMax = 1LL << 21;
 constexpr long long kNoKey = LLONG_MAX;
 
-struct Crop {
-  int sphere, box;
-  double c[3], r2, lo[3], hi[3];
-};
-
 struct Plane {
   double n[4];
 };
-
-__device__ __forceinline__ bool inside(const Crop& q, double x, double y, double z) {
-  if (q.sphere) {
-    const double dx = __dsub_rn(x, q.c[0]), dy = __dsub_rn(y, q.c[1]), dz = __dsub_rn(z, q.c[2]);
-    if (!(__dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz)) <= q.r2)) return false;
-  }
-  if (q.box) {
-    if (!(x >= q.lo[0] && x <= q.hi[0] && y >= q.lo[1] && y <= q.hi[1] && z >= q.lo[2] && z <= q.hi[2])) return false;
-  }
-  return true;
-}
 
 // signed distance ((nx x + ny y) + nz z) + d, uncontracted
 __device__ __forceinline__ double plane_r(double nx, double ny, double nz, double d, double x, double y, double z) {
@@ -72,64 +59,12 @@ __global__ void __launch_bounds__(kBlock) crop_kernel(const double* __restrict__
 }
 
 // ------------------------------------------------------------------------------------------------ ordered compaction
-// exclusive prefix of x over the block in thread order; *total = block sum.  s_w: kBlock/32 ints.
-__device__ __forceinline__ int block_scan(int x, int* s_w, int* total) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  int incl = x;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int v = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += v;
-  }
-  if (lane == 31) s_w[wid] = incl;
-  __syncthreads();
-  int before = 0, tot = 0;
-#pragma unroll
-  for (int w = 0; w < kBlock / 32; ++w) {
-    const int v = s_w[w];
-    before += w < wid ? v : 0;
-    tot += v;
-  }
-  *total = tot;
-  return before + incl - x;
-}
-
 __global__ void __launch_bounds__(kBlock) count_kernel(const unsigned char* __restrict__ flag, long long n, int* __restrict__ blk_cnt) {
   __shared__ int s_w[kBlock / 32];
   const long long i = (long long)blockIdx.x * kBlock + threadIdx.x;
   int total;
-  block_scan(i < n && flag[i] ? 1 : 0, s_w, &total);
+  block_scan<kBlock>(i < n && flag[i] ? 1 : 0, s_w, &total);
   if (threadIdx.x == 0) blk_cnt[blockIdx.x] = total;
-}
-
-__device__ __forceinline__ long long warp_incl(long long x, int lane) {
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const long long v = __shfl_up_sync(0xffffffffu, x, o);
-    if (lane >= o) x += v;
-  }
-  return x;
-}
-
-// one block: exclusive scan of the block counts in block order (chunks of 1024 with a 64-bit carry), and the total
-__global__ void __launch_bounds__(kScanThreads) scan_kernel(const int* __restrict__ blk_cnt, long long* __restrict__ blk_off,
-                                                            long long* __restrict__ total, int nblk) {
-  __shared__ long long s_w[32];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  long long carry = 0;
-  for (int c0 = 0; c0 < nblk; c0 += kScanThreads) {
-    const int b = c0 + threadIdx.x;
-    const long long v = b < nblk ? blk_cnt[b] : 0;
-    const long long iv = warp_incl(v, lane);
-    if (lane == 31) s_w[wid] = iv;
-    __syncthreads();
-    if (wid == 0) s_w[lane] = warp_incl(s_w[lane], lane);
-    __syncthreads();
-    if (b < nblk) blk_off[b] = carry + (wid ? s_w[wid - 1] : 0) + iv - v;
-    carry += s_w[31];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) *total = carry;
 }
 
 __global__ void __launch_bounds__(kBlock) emit_kernel(const double* __restrict__ pts, const unsigned char* __restrict__ flag, long long n,
@@ -139,7 +74,7 @@ __global__ void __launch_bounds__(kBlock) emit_kernel(const double* __restrict__
   const long long i = (long long)blockIdx.x * kBlock + threadIdx.x;
   const bool f = i < n && flag[i];
   int total;
-  const int r = block_scan(f ? 1 : 0, s_w, &total);
+  const int r = block_scan<kBlock>(f ? 1 : 0, s_w, &total);
   if (!f) return;
   const long long pos = blk_off[blockIdx.x] + r;
   idx[pos] = int(i);
@@ -308,37 +243,6 @@ __device__ __forceinline__ long long find_key(const long long* __restrict__ ukey
   return -1;
 }
 
-__global__ void __launch_bounds__(kBlock) uf_init_kernel(int* __restrict__ parent, long long m) {
-  const long long v = (long long)blockIdx.x * kBlock + threadIdx.x;
-  if (v < m) parent[v] = int(v);
-}
-
-// root of x with path halving.  Every parent pointer points to a smaller (or the same) index and only ever moves to an
-// ancestor, so the halving stores, racing with each other and with the hooks, keep a forest with the same roots.
-__device__ __forceinline__ int uf_find(volatile int* parent, int x) {
-  while (true) {
-    const int p = parent[x];
-    if (p == x) return x;
-    const int g = parent[p];
-    if (g != p) parent[x] = g;
-    x = g;
-  }
-}
-
-__device__ __forceinline__ void uf_unite(int* parent, int a, int b) {
-  volatile int* vp = parent;
-  while (true) {
-    a = uf_find(vp, a);
-    b = uf_find(vp, b);
-    if (a == b) return;
-    if (a > b) { const int s = a; a = b; b = s; }
-    // hook root b under the smaller root a; if b stopped being a root meanwhile, retry from its new parent
-    const int old = atomicCAS(parent + b, b, a);
-    if (old == b) return;
-    b = old;
-  }
-}
-
 // the 13 neighbours (da, db, dc) > (0, 0, 0) in lexicographic order have the larger packed keys, so they lie after v
 __global__ void __launch_bounds__(kBlock) vox_hook_kernel(const long long* __restrict__ ukeys, long long m, int* parent) {
   const long long v = (long long)blockIdx.x * kBlock + threadIdx.x;
@@ -351,16 +255,6 @@ __global__ void __launch_bounds__(kBlock) vox_hook_kernel(const long long* __res
     const long long u = find_key(ukeys, v + 1, m, (na << 42) | (nb << 21) | nc);
     if (u >= 0) uf_unite(parent, int(v), int(u));
   }
-}
-
-// one round of pointer jumping: parent[v] <- parent[parent[v]]
-__global__ void __launch_bounds__(kBlock) uf_jump_kernel(int* parent, long long m) {
-  const long long v = (long long)blockIdx.x * kBlock + threadIdx.x;
-  if (v >= m) return;
-  volatile int* vp = parent;
-  const int p = vp[v];
-  const int g = vp[p];
-  if (g != p) vp[v] = g;
 }
 
 __global__ void __launch_bounds__(kBlock) copy_label_kernel(const int* __restrict__ parent, long long m, int* __restrict__ label) {
@@ -425,19 +319,8 @@ extern "C" {
 
 int nero_objprep_crop(const double* pts, long long n, const double* sphere, const double* box, unsigned char* keep, void* stream) {
   if (!pts || !keep || n < 1 || n > kMaxN) return NERO_ERR_ARG;
-  Crop q{};
-  if (sphere) {
-    if (!(sphere[3] > 0.0) || !finite_n(sphere, 4)) return NERO_ERR_ARG;
-    q.sphere = 1;
-    q.c[0] = sphere[0]; q.c[1] = sphere[1]; q.c[2] = sphere[2];
-    q.r2 = sphere[3] * sphere[3];
-  }
-  if (box) {
-    for (int a = 0; a < 3; ++a)
-      if (!(box[a] <= box[3 + a])) return NERO_ERR_ARG;
-    q.box = 1;
-    for (int a = 0; a < 3; ++a) { q.lo[a] = box[a]; q.hi[a] = box[3 + a]; }
-  }
+  Crop q;
+  if (!make_crop(sphere, box, q)) return NERO_ERR_ARG;
   crop_kernel<<<nblocks(n), kBlock, 0, (cudaStream_t)stream>>>(pts, n, q, keep);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
@@ -448,7 +331,7 @@ int nero_objprep_compact_count(const unsigned char* flag, long long n, int* blk_
   const cudaStream_t s = (cudaStream_t)stream;
   const int nb = int(nblocks(n));
   count_kernel<<<nb, kBlock, 0, s>>>(flag, n, blk_cnt);
-  scan_kernel<<<1, kScanThreads, 0, s>>>(blk_cnt, blk_off, total, nb);
+  block_offsets<1>(blk_cnt, blk_off, total, nb, s);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
@@ -510,11 +393,9 @@ int nero_objprep_above(const double* pts, long long n, const unsigned char* keep
 int nero_objprep_voxel_components(const long long* ukeys, long long m, int* parent, int* label, void* stream) {
   if (!ukeys || !parent || !label || m < 1 || m > kMaxN) return NERO_ERR_ARG;
   const cudaStream_t s = (cudaStream_t)stream;
-  uf_init_kernel<<<nblocks(m), kBlock, 0, s>>>(parent, m);
+  uf_init(parent, m, s);
   vox_hook_kernel<<<nblocks(m), kBlock, 0, s>>>(ukeys, m, parent);
-  int rounds = 1;                        // ceil(log2 m) + 1: a tree has depth < m
-  while ((1LL << (rounds - 1)) < m) ++rounds;
-  for (int r = 0; r < rounds; ++r) uf_jump_kernel<<<nblocks(m), kBlock, 0, s>>>(parent, m);
+  uf_flatten(parent, m, s);
   copy_label_kernel<<<nblocks(m), kBlock, 0, s>>>(parent, m, label);
   NERO_LAUNCH_CHECK();
   return NERO_OK;

@@ -4,8 +4,8 @@
 //   raster     one thread per uv triangle over its texel bounding box: uv snapped to 1/256 texel, exact int64 edge functions
 //              with the top-left rule (either winding; zero-area triangles own nothing).  owner = atomicMin(triangle id), so
 //              the map is deterministic even where triangles overlap; cover counts them.
-//   compact    ordered compaction of the covered texels in row-major order: count -> one-block scan -> emit, as in
-//              k_eval.cu.  emit interpolates the mesh positions in fp32 with the barycentrics of the same edge functions.
+//   compact    ordered compaction of the covered texels in row-major order: count -> one-block scan -> emit
+//              (compact.cuh).  emit interpolates the mesh positions in fp32 with the barycentrics of the same edge functions.
 //   encode     linear_to_srgb in fp64 as numpy evaluates it (no contraction), x 255, truncated to uint8.
 //   inpaint    search texels (covered, Manhattan distance <= 3 from an uncovered texel or the border), a 16x16 tile map of
 //              them, then per uncovered texel a ring-by-ring scan of the radius-32 window for the nearest search texel.
@@ -14,6 +14,7 @@
 // No atomics combine values except the order-free atomicMin / count of the raster, so every output is bit-identical from
 // run to run.
 #include "common.cuh"
+#include "compact.cuh"
 #include "../../include/nero_texmap.h"
 
 namespace nero {
@@ -92,30 +93,6 @@ __global__ void __launch_bounds__(128) raster_kernel(const float* __restrict__ v
 constexpr int kTxThreads = 256;
 constexpr int kTxSub = 4;
 constexpr int kTxTile = kTxThreads * kTxSub;   // keep in step with include/nero_texmap.h (nblk)
-constexpr int kTxScanThreads = 1024;
-
-// exclusive prefix of x over the block in thread order; *total = block sum.  s_w: kTxThreads/32 ints.  (k_eval.cu's scan.)
-__device__ __forceinline__ int tx_block_scan(int x, int* s_w, int* total) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  int incl = x;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int v = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += v;
-  }
-  if (lane == 31) s_w[wid] = incl;
-  __syncthreads();
-  int before = 0, tot = 0;
-#pragma unroll
-  for (int w = 0; w < kTxThreads / 32; ++w) {
-    const int v = s_w[w];
-    before += w < wid ? v : 0;
-    tot += v;
-  }
-  __syncthreads();
-  *total = tot;
-  return before + incl - x;
-}
 
 __device__ __forceinline__ bool tx_covered(const unsigned* owner, long long L, long long N) {
   return L < N && __ldg(owner + L) != kNoOwner;
@@ -127,37 +104,8 @@ __global__ void __launch_bounds__(kTxThreads) texel_count_kernel(const unsigned*
   int n = 0;
   for (int s = 0; s < kTxSub; ++s) n += tx_covered(owner, base + s * kTxThreads + threadIdx.x, N) ? 1 : 0;
   int total;
-  tx_block_scan(n, s_w, &total);
+  block_scan<kTxThreads>(n, s_w, &total);
   if (threadIdx.x == 0) blk_cnt[blockIdx.x] = total;
-}
-
-__device__ __forceinline__ long long tx_warp_incl(long long x, int lane) {
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const long long v = __shfl_up_sync(0xffffffffu, x, o);
-    if (lane >= o) x += v;
-  }
-  return x;
-}
-
-__global__ void __launch_bounds__(kTxScanThreads) texel_scan_kernel(const int* __restrict__ blk_cnt, long long* __restrict__ blk_off,
-                                                                    long long* __restrict__ total, int nblk) {
-  __shared__ long long s_w[32];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  long long carry = 0;
-  for (int c0 = 0; c0 < nblk; c0 += kTxScanThreads) {
-    const int b = c0 + threadIdx.x;
-    const long long v = b < nblk ? blk_cnt[b] : 0;
-    const long long iv = tx_warp_incl(v, lane);
-    if (lane == 31) s_w[wid] = iv;
-    __syncthreads();
-    if (wid == 0) s_w[lane] = tx_warp_incl(s_w[lane], lane);
-    __syncthreads();
-    if (b < nblk) blk_off[b] = carry + (wid ? s_w[wid - 1] : 0) + iv - v;
-    carry += s_w[31];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) *total = carry;
 }
 
 __global__ void __launch_bounds__(kTxThreads) texel_emit_kernel(const unsigned* __restrict__ owner, long long N, int width, int height,
@@ -172,7 +120,7 @@ __global__ void __launch_bounds__(kTxThreads) texel_emit_kernel(const unsigned* 
     const long long L = base + s * kTxThreads + threadIdx.x;
     const bool keep = tx_covered(owner, L, N);
     int total;
-    const int off = tx_block_scan(keep ? 1 : 0, s_w, &total);
+    const int off = block_scan<kTxThreads>(keep ? 1 : 0, s_w, &total);
     if (keep) {
       const int t = int(__ldg(owner + L));
       const SnapTri q = snap_tri(vt, ft, t, width, height);
@@ -333,7 +281,7 @@ int nero_tex_compact_count(const unsigned int* owner, int width, int height, int
   int nblk;
   if (!owner || !blk_cnt || !blk_off || !total || !tx_grid(width, height, N, nblk)) return NERO_ERR_ARG;
   texel_count_kernel<<<nblk, kTxThreads, 0, st>>>(owner, N, blk_cnt);
-  texel_scan_kernel<<<1, kTxScanThreads, 0, st>>>(blk_cnt, blk_off, total, nblk);
+  block_offsets<1>(blk_cnt, blk_off, total, nblk, st);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }

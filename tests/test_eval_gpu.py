@@ -101,6 +101,15 @@ def test_points_match_oracle_order_and_values():
     ref = np.concatenate([OE.depth_to_points(d.cpu().numpy(), d.cpu().numpy() > 0, K, p) for d, p, K in zip(depths, poses, Ks)], 0)
     assert got.shape == ref.shape and got.shape[0] > 100
     np.testing.assert_allclose(got, ref, rtol=1e-6, atol=1e-6 * np.abs(ref).max())
+    # three 640 x 640 views: 1 228 800 pixels in 1200 blocks, so the block offsets carry a sum across their 1024-block chunks
+    K = np.asarray([[800.0, 0, 320], [0, 800.0, 320], [0, 0, 1]], np.float32)
+    poses = [camera(i)[0] for i in range(3)]
+    depths = torch.stack([r.render(p, K, 640, 640) for p in poses])
+    assert (depths.reshape(-1)[:1024 * 1024] > 0).any() and (depths.reshape(-1)[1024 * 1024:] > 0).any()
+    got = E.depth_to_points_cuda(depths, poses, [K] * 3).cpu().numpy()
+    ref = np.concatenate([OE.depth_to_points(d.cpu().numpy(), d.cpu().numpy() > 0, K, p) for d, p in zip(depths, poses)], 0)
+    assert got.shape == ref.shape
+    np.testing.assert_allclose(got, ref, rtol=1e-6, atol=1e-6 * np.abs(ref).max())
     # the ground-truth mask (-inf, 14.5) of a 16-bit depth map
     raw = np.random.RandomState(0).randint(0, 65536, (37, 29)).astype(np.uint16)
     d = raw.astype(np.float32) / 65535 * 15

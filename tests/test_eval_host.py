@@ -211,7 +211,7 @@ def test_eval_kernels_do_not_spill():
     kernels = re.findall(r"Compiling entry function '(\w+)'.*?(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads",
                          out.stderr, re.S)
     names = {k[0] for k in kernels}
-    for want in ('depth_render_kernel', 'points_count_kernel', 'points_scan_kernel', 'points_emit_kernel', 'voxel_keys_kernel',
+    for want in ('depth_render_kernel', 'points_count_kernel', 'block_offsets_kernel', 'points_emit_kernel', 'voxel_keys_kernel',
                  'voxel_mean_kernel', 'nearest_kernel'):
         assert any(want in n for n in names), want
     for name, stack, st, ld in kernels:
