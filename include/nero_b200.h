@@ -72,6 +72,10 @@ typedef struct nero_chain_params {
   const float* A0; int lda0; int k_valid0;
   int n_layers; const int* m_ptr; int m_cap;
   nero_chain_layer L[10];
+  /* phase_clk: NULL, except with the diagnostic build compiled with NERO_CHAIN_PHASES (tools/chain_phases.py), where it
+   * points to zeroed device memory of 132 * (2 * 10 * 5 + 2) counters: the SM cycles each warpgroup spent in each phase
+   * of each layer, then per CTA its cycles and globaltimer nanoseconds (k_gemm_chain.cu).  The product build ignores it. */
+  unsigned long long* phase_clk;
 } nero_chain_params;
 int nero_chain(const void* chain_params_host, void* stream);
 /* Y[i,:] += a[i*lda] * X[i,:] */

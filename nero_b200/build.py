@@ -7,6 +7,9 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libnero_b200.so')
+# diagnostic build: the fused chain kernel with its phase timers (tools/chain_phases.py loads it through NERO_LIB)
+PHASES_LIB = os.path.join(HERE, 'libnero_b200_phases.so')
+PHASES_FLAGS = ('-DNERO_CHAIN_PHASES',)
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 # diagnostic 338 (two declarations of one extern "C" function with different parameters) is only a warning for a
@@ -19,10 +22,10 @@ def sources():
     return sorted(glob.glob(os.path.join(CSRC, '*.cu')))
 
 
-def needs_build():
-    if not os.path.exists(LIB):
+def needs_build(lib=LIB):
+    if not os.path.exists(lib):
         return True
-    t = os.path.getmtime(LIB)
+    t = os.path.getmtime(lib)
     deps = sources() + glob.glob(os.path.join(CSRC, '*.cuh')) + glob.glob(os.path.join(HERE, '..', 'include', '*.h'))
     return any(os.path.getmtime(d) > t for d in deps)
 
@@ -50,6 +53,13 @@ def build(force=False, verbose=False, extra_flags=(), lib_out=None):
     cmd = [NVCC] + ARCH + ['-shared', '-o', lib_out or LIB] + objs + ['-lcudart']
     subprocess.check_call(cmd)
     return lib_out or LIB
+
+
+def build_phases():
+    """The diagnostic library with the chain kernel's phase timers; never the one the package loads by default."""
+    if needs_build(PHASES_LIB):
+        build(extra_flags=PHASES_FLAGS, lib_out=PHASES_LIB)
+    return PHASES_LIB
 
 
 if __name__ == '__main__':

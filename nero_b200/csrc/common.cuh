@@ -91,5 +91,9 @@ NERO_HD void split_bf16(float x, __nv_bfloat16& hi, __nv_bfloat16& lo) {
 __host__ __device__ __forceinline__ uint32_t sw128_offset(uint32_t r, uint32_t kk) {
   return r * 128u + ((((kk >> 3) ^ (r & 7u)) << 4) | ((kk & 7u) << 1));
 }
+// byte offset of element (row r, k index kk in [0,32)) inside one K-major SWIZZLE_64B operand tile
+__host__ __device__ __forceinline__ uint32_t sw64_offset(uint32_t r, uint32_t kk) {
+  return r * 64u + ((((kk >> 3) ^ ((r >> 1) & 3u)) << 4) | ((kk & 7u) << 1));
+}
 
 }  // namespace nero

@@ -88,12 +88,15 @@ __device__ __forceinline__ float2 ld2(const float* __restrict__ g, int ld, long 
 inline bool pair_aligned(const float* g, int ld) {
   return !g || ((reinterpret_cast<uintptr_t>(g) & 7) == 0 && (ld & 1) == 0);
 }
+// Written as three independently guarded stores rather than early returns, so that the compiler predicates them and the
+// epilogues' unrolled pairs stay one basic block it can schedule across.
 __device__ __forceinline__ void st2(float* __restrict__ g, int ld, long row, int col, int lim, bool ok, float a, float b) {
-  if (!ok || !g || col >= lim) return;
+  const bool in0 = ok && g && col < lim, in1 = in0 && col + 1 < lim;
   float* q = g + row * ld + col;
-  if (col + 1 < lim && (reinterpret_cast<uintptr_t>(q) & 7) == 0) { __stcs(reinterpret_cast<float2*>(q), make_float2(a, b)); return; }
-  __stcs(q, a);
-  if (col + 1 < lim) __stcs(q + 1, b);
+  const bool pair = in1 && (reinterpret_cast<uintptr_t>(q) & 7) == 0;
+  if (pair) __stcs(reinterpret_cast<float2*>(q), make_float2(a, b));
+  if (in0 && !pair) __stcs(q, a);
+  if (in1 && !pair) __stcs(q + 1, b);
 }
 
 // operands of the epilogue of one layer (nero_linear / one layer of nero_chain; see include/nero_b200.h)

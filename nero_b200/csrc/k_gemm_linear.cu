@@ -3,8 +3,9 @@
 //  * A is fp32 row-major in HBM.  All 256 threads load a 128 x 64 chunk of it with coalesced float4, split every value into
 //    bf16 hi + lo (packed cvt.rn.bf16x2) and store both planes in the K-major SWIZZLE_128B layout wgmma reads.  The loads
 //    of chunk c + 1 are in flight while the MMAs of chunk c run (two smem stages).
-//  * W is pre-split and pre-swizzled once per step by nero_prep_weight (k_weights.cu) into the exact shared-memory image,
-//    so a K-chunk of it is ONE cp.async.bulk (UBLKCP) from L2, completing on an mbarrier.
+//  * W is pre-split and pre-swizzled once per step by nero_prep_weight (k_weights.cu) into the exact shared-memory image
+//    (32-wide K chunks, SWIZZLE_64B), so a 64-wide K chunk of it is ONE cp.async.bulk (UBLKCP) from L2, completing on an
+//    mbarrier.
 //  * Two warpgroups, 64 rows each, issue wgmma.m64nNk16 (bf16 x bf16 -> fp32 registers), three per k-step (split-bf16,
 //    gemm_common.cuh); N = the padded layer width (16 .. 256), so one instruction covers the whole output row range.
 //  * The epilogue runs on the accumulator registers (pairs of adjacent columns, 8-byte accesses: every 32-byte sector a
@@ -38,7 +39,7 @@ constexpr int kLinearThreads = 256;
 constexpr uint32_t kABytes = BM * 128;           // one bf16 plane of an A chunk (128 rows x 64 K, 16 KB)
 
 template <int NPAD> struct LinCfg {
-  static constexpr uint32_t b_plane = NPAD * 128;
+  static constexpr uint32_t b_plane = NPAD * 128;   // the hi and lo planes of one 32-wide K chunk of W
   static constexpr uint32_t stage_bytes = 2 * kABytes + 2 * b_plane;
   static constexpr uint32_t smem_bytes = 2 * stage_bytes + 1024 /*align*/ + 64 /*barriers*/;
 };
@@ -99,13 +100,16 @@ __global__ void __launch_bounds__(kLinearThreads, 1) gemm_linear_kernel(const Li
       __syncthreads();
       mbar_wait(&full[s], (g >> 1) & 1);
       const uint32_t a_hi = smem_u32(st) + wg * 64 * 128, a_lo = a_hi + kABytes;
-      const uint32_t b_hi = smem_u32(st) + 2 * kABytes, b_lo = b_hi + Cfg::b_plane;
+      // the weight chunk is two 32-wide K chunks, each a hi and a lo plane of NPAD rows x 64 B (SWIZZLE_64B)
+      const uint32_t b0 = smem_u32(st) + 2 * kABytes;
       fence_regs<NPAD / 2>(acc);
       wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < 4; ++k)
-        mma_split3<NPAD, 0, 0>(acc, make_desc_k_sw128(a_hi + 32 * k), make_desc_k_sw128(a_lo + 32 * k), make_desc_k_sw128(b_hi + 32 * k),
-                               make_desc_k_sw128(b_lo + 32 * k), (c | k) != 0);
+      for (int k = 0; k < 4; ++k) {
+        const uint32_t b_hi = b0 + (k >> 1) * Cfg::b_plane + 32 * (k & 1), b_lo = b_hi + Cfg::b_plane / 2;
+        mma_split3<NPAD, 0, 0>(acc, make_desc_k_sw128(a_hi + 32 * k), make_desc_k_sw128(a_lo + 32 * k), make_desc_k_sw64(b_hi),
+                               make_desc_k_sw64(b_lo), (c | k) != 0);
+      }
       wgmma_commit();
       wgmma_wait<1>();
       fence_regs<NPAD / 2>(acc);

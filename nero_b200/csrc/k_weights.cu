@@ -4,8 +4,9 @@
 // writes, for rows [row0, row0+nrows) of the layer,
 //   * img_f : the forward tensor-core operand image  (tile rows = output features, K = input layout columns)
 //   * img_t : the transposed image for input-gradient GEMMs (tile rows = input layout columns, K = output features)
-// both as split-bf16 (hi plane, lo plane) per 64-wide K chunk in the K-major SWIZZLE_128B shared-memory layout,
-// so the GEMM kernels fetch a chunk with one bulk copy.  `kmap` places reference input column k at column
+// both as split-bf16 (hi plane, lo plane) per 32-wide K chunk in the K-major SWIZZLE_64B shared-memory layout,
+// so the GEMM kernels fetch a chunk (or two adjacent ones) with one bulk copy.  32-wide chunks let the fused chain stream
+// its weights in 16 KB stages of 128 rows (k_gemm_chain.cu).  `kmap` places reference input column k at column
 // kmap[k] of the (padded / re-ordered) activation layout the kernels actually use; `in_scale` folds constant
 // input scalings.  Images must be zero-initialised once (padding stays zero).
 //
@@ -28,13 +29,13 @@ __device__ __forceinline__ float block_sum(float v, float* sh) {
 }
 
 __device__ __forceinline__ void img_store(uint8_t* img, int rows_pad, int r, int kcol, float w) {
-  const int c = kcol >> 6, kk = kcol & 63;
-  uint8_t* base = img + size_t(c) * 2 * rows_pad * 128;
+  const int c = kcol >> 5, kk = kcol & 31;
+  uint8_t* base = img + size_t(c) * 2 * rows_pad * 64;
   __nv_bfloat16 hi, lo;
   split_bf16(w, hi, lo);
-  const uint32_t off = sw128_offset(r, kk);
+  const uint32_t off = sw64_offset(r, kk);
   *reinterpret_cast<__nv_bfloat16*>(base + off) = hi;
-  *reinterpret_cast<__nv_bfloat16*>(base + size_t(rows_pad) * 128 + off) = lo;
+  *reinterpret_cast<__nv_bfloat16*>(base + size_t(rows_pad) * 64 + off) = lo;
 }
 
 __device__ __forceinline__ void prep_weight_row(int r, const float* __restrict__ v, const float* __restrict__ g, int K, int row0,

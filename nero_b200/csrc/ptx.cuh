@@ -17,6 +17,10 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 __device__ __forceinline__ void sts_u32(uint32_t addr, uint32_t v) {
   asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v));
 }
+// the same store, executed only where `on` holds (a predicated instruction, not a branch)
+__device__ __forceinline__ void sts_u32_if(uint32_t addr, uint32_t v, bool on) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %2, 0;\n\t@p st.shared.b32 [%0], %1;\n\t}" ::"r"(addr), "r"(v), "r"(uint32_t(on)));
+}
 
 // ------------------------------------------------------------------ mbarrier
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
@@ -55,6 +59,13 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 // make generic-proxy smem writes visible to the async proxy (wgmma / bulk copies read smem through it)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+}
+// shared-memory counter: adds v and returns the old value, with acquire-release ordering at CTA scope (the accesses
+// ordered before one thread's add are visible to a thread whose later add reads its result)
+__device__ __forceinline__ uint32_t atom_add_acq_rel_smem(uint32_t addr, uint32_t v) {
+  uint32_t old;
+  asm volatile("atom.acq_rel.cta.shared::cta.add.u32 %0, [%1], %2;" : "=r"(old) : "r"(addr), "r"(v) : "memory");
+  return old;
 }
 // named barrier over `count` threads (ids 1..15; 0 is __syncthreads)
 __device__ __forceinline__ void named_bar(int id, int count) {
@@ -110,6 +121,15 @@ __device__ __forceinline__ uint64_t make_desc_k_sw128(uint32_t smem_addr) {
   d |= static_cast<uint64_t>(1) << 16;
   d |= static_cast<uint64_t>(1024 >> 4) << 32;
   d |= static_cast<uint64_t>(1) << 62;
+  return d;
+}
+// K-major operand tile, 64-byte swizzle: rows are 64 B (32 bf16) apart, 8-row groups 512 B apart (LBO unused).
+__device__ __forceinline__ uint64_t make_desc_k_sw64(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
+  d |= static_cast<uint64_t>(1) << 16;
+  d |= static_cast<uint64_t>(512 >> 4) << 32;
+  d |= static_cast<uint64_t>(2) << 62;
   return d;
 }
 // MN-major operand tile, 128-byte swizzle (canonical layout ((8,8,m),(8,k)):((1,8,LBO),(64,SBO)) in bf16 elements): an

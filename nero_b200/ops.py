@@ -409,6 +409,7 @@ def chain_layer(layer: PreparedLayer, kind, ncol_out, *, transposed=False, save:
 
 
 PROFILE = None   # bench.py: list collecting (tag, event0, event1, flops_per_row, m_ptr_addr, m_cap) per chain launch
+CHAIN_PHASES = None   # tools/chain_phases.py: int64 device counters the NERO_CHAIN_PHASES build adds each launch's phases to
 
 
 def chain(A0: Mat, k_valid0, layers, m_ptr=None, m_cap=None, tag=''):
@@ -419,6 +420,7 @@ def chain(A0: Mat, k_valid0, layers, m_ptr=None, m_cap=None, tag=''):
     assert 1 <= len(layers) <= len(P.L)
     P.A0, P.lda0, P.k_valid0 = _addr(A0), A0.ld, ceil_div(k_valid0, 4) * 4
     P.n_layers, P.m_ptr, P.m_cap = len(layers), _addr(m_ptr), m_cap
+    P.phase_clk = _addr(CHAIN_PHASES)
     keep = []
     for i, d in enumerate(layers):
         lay, L = d['layer'], P.L[i]
