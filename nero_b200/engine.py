@@ -19,10 +19,14 @@ import numpy as np
 import torch
 
 from . import ops
-from .ops import Mat, K, linear, wgrad, chain, chain_layer as CL, ACT_NONE, ACT_SOFTPLUS100, ACT_RELU, ACT_SIGMOID, ACT_EXPCLAMP, EPI_MUL_DACT, EPI_TANGENT
+# chain is not called here (the passes launch through ops.mlp); it stays bound, like in material.py, because the GEMM census
+# wraps chain / linear / wgrad by patching these names in ops, engine and material
+from .ops import Mat, K, linear, wgrad, chain, mlp, chain_layer as CL, ACT_NONE, ACT_RELU, ACT_SIGMOID, ACT_EXPCLAMP, EPI_MUL_DACT
 from .ops import EK_BIAS_SOFTPLUS, EK_BIAS_RELU, EK_BIAS_GENERIC, EK_DACT_SOFTPLUS, EK_DACT_RELU, EK_DACT_NONE, EK_TANGENT
 
-USE_CHAIN = True    # fused MLP-chain kernel (k_gemm_chain.cu); False = one nero_linear launch per layer
+# Every stage-I MLP pass is stated once, as the layer list of the fused chain kernel (k_gemm_chain.cu).  True: ops.mlp runs
+# it as nero_chain launches; False: ops.mlp expands the same list into one nero_linear launch per layer
+USE_CHAIN = True
 
 INV_SQRT2 = 0.7071067811865476
 SQRT2 = 1.4142135623730951
@@ -137,46 +141,26 @@ class Predictor:
 
     def forward(self, A, acts, out, m_ptr, m_cap):
         L = self.layers
-        if USE_CHAIN:
-            tail = [CL(L[1], EK_BIAS_RELU, 256, save=Mat(acts[1])), CL(L[2], EK_BIAS_RELU, 256, save=Mat(acts[2])),
-                    CL(L[3], EK_BIAS_GENERIC, self.n_out, save=out, act=self.act, act_param=self.act_param)]
-            if L[0].k_chunks <= 4:
-                chain(A, L[0].k_valid, [CL(L[0], EK_BIAS_RELU, 256, save=Mat(acts[0]))] + tail, m_ptr, m_cap)
-            else:
-                linear(A, L[0], Mat(acts[0]), 256, act=ACT_RELU, m_ptr=m_ptr, m_cap=m_cap)
-                chain(Mat(acts[0]), 256, tail, m_ptr, m_cap)
-            return
-        linear(A, L[0], Mat(acts[0]), 256, act=ACT_RELU, m_ptr=m_ptr, m_cap=m_cap)
-        linear(Mat(acts[0]), L[1], Mat(acts[1]), 256, act=ACT_RELU, m_ptr=m_ptr, m_cap=m_cap)
-        linear(Mat(acts[1]), L[2], Mat(acts[2]), 256, act=ACT_RELU, m_ptr=m_ptr, m_cap=m_cap)
-        linear(Mat(acts[2]), L[3], out, self.n_out, act=self.act, act_param=self.act_param, m_ptr=m_ptr, m_cap=m_cap)
+        mlp(A, [CL(L[0], EK_BIAS_RELU, 256, save=Mat(acts[0])), CL(L[1], EK_BIAS_RELU, 256, save=Mat(acts[1])),
+                CL(L[2], EK_BIAS_RELU, 256, save=Mat(acts[2])),
+                CL(L[3], EK_BIAS_GENERIC, self.n_out, save=out, act=self.act, act_param=self.act_param)], m_ptr, m_cap, fused=USE_CHAIN)
 
-    def backward(self, ws, dpre, A, acts, dHa, dHb, m_ptr, m_cap, dX=None, dx_ncol=0, dx_addend=None, dHc=None):
-        """dpre: Mat over the pre-activation gradient of the output (n_out columns)."""
+    def backward(self, ws, dpre, A, acts, dH, m_ptr, m_cap, dX=None, dx_ncol=0, dx_addend=None):
+        """dpre: Mat over the pre-activation gradient of the output (n_out columns); dH: three [., 256] buffers that receive
+        the pre-activation gradients of the hidden layers 2, 1, 0."""
         L, P = self.layers, self.pl
         g = lambda i: (P[i].weight_v.grad, P[i].weight_g.grad, P[i].bias.grad)
         kw = dict(m_ptr=m_ptr, m_cap=m_cap)
-        if USE_CHAIN and dHc is not None:
-            ls = [CL(L[3], EK_DACT_RELU, 256, transposed=True, H=Mat(acts[2]), save=Mat(dHa)),
-                  CL(L[2], EK_DACT_RELU, 256, transposed=True, H=Mat(acts[1]), save=Mat(dHb)),
-                  CL(L[1], EK_DACT_RELU, 256, transposed=True, H=Mat(acts[0]), save=Mat(dHc))]
-            if dX is not None:
-                ls.append(CL(L[0], EK_DACT_NONE, dx_ncol, transposed=True, addend=dx_addend, save=dX))
-            chain(dpre, self.n_out, ls, m_ptr, m_cap)
-            wgrad(ws, dpre, self.n_out, Mat(acts[2]), 256, L[3], *g(3), **kw)
-            wgrad(ws, Mat(dHa), 256, Mat(acts[1]), 256, L[2], *g(2), **kw)
-            wgrad(ws, Mat(dHb), 256, Mat(acts[0]), 256, L[1], *g(1), **kw)
-            wgrad(ws, Mat(dHc), 256, A, L[0].k_valid, L[0], *g(0), **kw)
-            return
-        linear(dpre, L[3], Mat(dHa), 256, transposed=True, mode=EPI_MUL_DACT, H=Mat(acts[2]), dact=ACT_RELU, **kw)
-        wgrad(ws, dpre, self.n_out, Mat(acts[2]), 256, L[3], *g(3), **kw)
-        linear(Mat(dHa), L[2], Mat(dHb), 256, transposed=True, mode=EPI_MUL_DACT, H=Mat(acts[1]), dact=ACT_RELU, **kw)
-        wgrad(ws, Mat(dHa), 256, Mat(acts[1]), 256, L[2], *g(2), **kw)
-        linear(Mat(dHb), L[1], Mat(dHa), 256, transposed=True, mode=EPI_MUL_DACT, H=Mat(acts[0]), dact=ACT_RELU, **kw)
-        wgrad(ws, Mat(dHb), 256, Mat(acts[0]), 256, L[1], *g(1), **kw)
+        ls = [CL(L[3], EK_DACT_RELU, 256, transposed=True, H=Mat(acts[2]), save=Mat(dH[0])),
+              CL(L[2], EK_DACT_RELU, 256, transposed=True, H=Mat(acts[1]), save=Mat(dH[1])),
+              CL(L[1], EK_DACT_RELU, 256, transposed=True, H=Mat(acts[0]), save=Mat(dH[2]))]
         if dX is not None:
-            linear(Mat(dHa), L[0], dX, dx_ncol, transposed=True, mode=EPI_MUL_DACT, addend=dx_addend, **kw)
-        wgrad(ws, Mat(dHa), 256, A, L[0].k_valid, L[0], *g(0), **kw)
+            ls.append(CL(L[0], EK_DACT_NONE, dx_ncol, transposed=True, addend=dx_addend, save=dX))
+        mlp(dpre, ls, m_ptr, m_cap, fused=USE_CHAIN)
+        wgrad(ws, dpre, self.n_out, Mat(acts[2]), 256, L[3], *g(3), **kw)
+        wgrad(ws, Mat(dH[0]), 256, Mat(acts[1]), 256, L[2], *g(2), **kw)
+        wgrad(ws, Mat(dH[1]), 256, Mat(acts[0]), 256, L[1], *g(1), **kw)
+        wgrad(ws, Mat(dH[2]), 256, A, L[0].k_valid, L[0], *g(0), **kw)
 
 
 class SdfNet:
@@ -201,73 +185,38 @@ class SdfNet:
         for l in self.L + [self.L8f, self.L8s]:
             l.prep()
 
-    def hidden_forward(self, X0, Hs, H4buf, m_ptr, m_cap, save=True, heads=None):
-        """X0 [.,64] -> Hs[k] = input of layer k+1 (k = 0..7); the output of lin3 goes into H4buf[:, :217] scaled by
-        1/sqrt2 next to the pre-filled PE/sqrt2 tail (skip concat, field.py:139-140)."""
-        kw = dict(act=ACT_SOFTPLUS100, m_ptr=m_ptr, m_cap=m_cap)
-        if USE_CHAIN:
-            sv = (lambda t: Mat(t)) if save else (lambda t: None)
-            ls = [CL(self.L[0], EK_BIAS_SOFTPLUS, 256, save=sv(Hs[0])), CL(self.L[1], EK_BIAS_SOFTPLUS, 256, save=sv(Hs[1])),
-                  CL(self.L[2], EK_BIAS_SOFTPLUS, 256, save=sv(Hs[2])),
-                  CL(self.L[3], EK_BIAS_SOFTPLUS, 217, oscale=INV_SQRT2, save=sv(H4buf), csrc=Mat(H4buf)),
-                  CL(self.L[4], EK_BIAS_SOFTPLUS, 256, save=sv(Hs[4])), CL(self.L[5], EK_BIAS_SOFTPLUS, 256, save=sv(Hs[5])),
-                  CL(self.L[6], EK_BIAS_SOFTPLUS, 256, save=sv(Hs[6])), CL(self.L[7], EK_BIAS_SOFTPLUS, 256, save=sv(Hs[7]))]
-            chain(Mat(X0), self.L[0].k_valid, ls + (heads or []), m_ptr, m_cap, tag='sdf_forward' if save else 'sdf_forward_nosave')
-            return
-        linear(Mat(X0), self.L[0], Mat(Hs[0]), 256, **kw)
-        linear(Mat(Hs[0]), self.L[1], Mat(Hs[1]), 256, **kw)
-        linear(Mat(Hs[1]), self.L[2], Mat(Hs[2]), 256, **kw)
-        linear(Mat(Hs[2]), self.L[3], Mat(H4buf), 217, oscale=INV_SQRT2, **kw)
-        linear(Mat(H4buf), self.L[4], Mat(Hs[4]), 256, **kw)
-        linear(Mat(Hs[4]), self.L[5], Mat(Hs[5]), 256, **kw)
-        linear(Mat(Hs[5]), self.L[6], Mat(Hs[6]), 256, **kw)
-        linear(Mat(Hs[6]), self.L[7], Mat(Hs[7]), 256, **kw)
+    def hidden_forward(self, X0, Hs, H4buf, m_ptr, m_cap, save=True, heads=()):
+        """X0 [.,64] -> Hs[k] = input of layer k+1 (k = 0..7), then the `heads` on Hs[7]; the output of lin3 goes into
+        H4buf[:, :217] scaled by 1/sqrt2 next to the pre-filled PE/sqrt2 tail (skip concat, field.py:139-140).
+        save=False: the fused chain stores only the heads' outputs (the per-layer path still writes Hs)."""
+        ls = [CL(self.L[k], EK_BIAS_SOFTPLUS, 256, save=Mat(Hs[k]), store=save) for k in (0, 1, 2)]
+        ls.append(CL(self.L[3], EK_BIAS_SOFTPLUS, 217, oscale=INV_SQRT2, save=Mat(H4buf), csrc=Mat(H4buf), store=save))
+        ls += [CL(self.L[k], EK_BIAS_SOFTPLUS, 256, save=Mat(Hs[k]), store=save) for k in (4, 5, 6, 7)]
+        mlp(Mat(X0), ls + list(heads), m_ptr, m_cap, tag='sdf_forward' if save else 'sdf_forward_nosave', fused=USE_CHAIN)
 
     def sdf_only(self, X0, SA, SB, SC, out, m_ptr, m_cap):
         """Forward-only SDF value (sampling / occlusion march): hidden stack in 3 rotating buffers, last layer row 0 only."""
-        Hs = [SA, SB, SA, SC, SA, SB, SA, SB]
-        if USE_CHAIN:
-            self.hidden_forward(X0, Hs, SC, m_ptr, m_cap, save=False,
-                                heads=[CL(self.L8s, EK_BIAS_GENERIC, 1, save=Mat(out), write_a=False)])
-            return
-        self.hidden_forward(X0, Hs, SC, m_ptr, m_cap)
-        linear(Mat(SB), self.L8s, Mat(out), 1, m_ptr=m_ptr, m_cap=m_cap)
+        self.hidden_forward(X0, [SA, SB, SA, SC, SA, SB, SA, SB], SC, m_ptr, m_cap, save=False,
+                            heads=[CL(self.L8s, EK_BIAS_GENERIC, 1, save=Mat(out), write_a=False)])
 
     # ---- training path on the compacted inner samples --------------------------------------------------
     def forward_with_gradient(self, w, m_ptr, m_cap):
-        H = w['H']   # H[1..8]; H[4] has the PE/sqrt2 tail pre-filled by ray_fill
-        Hs = [H[1], H[2], H[3], H[4], H[5], H[6], H[7], H[8]]
-        kw = dict(m_ptr=m_ptr, m_cap=m_cap)
-        V = w['V']
-        if USE_CHAIN:
-            self.hidden_forward(w['X0'], Hs, H[4], m_ptr, m_cap,
-                                heads=[CL(self.L8f, EK_BIAS_GENERIC, 256, save=Mat(w['Y8']), write_a=False),
-                                       CL(self.L8s, EK_BIAS_GENERIC, 1, save=Mat(w['Y8'], Y8_SDF), write_a=False)])
-            K('nero_dact_times_row', H[8], 256, self.L8s.w_eff, V[7], 256, 256, m_ptr, m_cap)
-            ls = []
-            for k in range(7, 0, -1):
-                if k == 4:
-                    ls.append(CL(self.L[4], EK_DACT_SOFTPLUS, 256, transposed=True, oscale=INV_SQRT2, H=Mat(H[4]), hscale=SQRT2,
-                                 ncol_main=217, tail=Mat(w['USKIP']), save=Mat(V[3])))
-                else:
-                    ls.append(CL(self.L[k], EK_DACT_SOFTPLUS, 256, transposed=True, H=Mat(H[k]), save=Mat(V[k - 1])))
-            ls.append(CL(self.L[0], EK_DACT_NONE, 39, transposed=True, save=Mat(w['U0'])))
-            chain(Mat(V[7]), 256, ls, m_ptr, m_cap, tag='sdf_reverse_sweep')
-            K('nero_pe_grad', w['X0'], 64, w['U0'], 64, w['USKIP'], 64, w['G'], m_ptr, m_cap)
-            return
-        self.hidden_forward(w['X0'], Hs, H[4], m_ptr, m_cap)
-        linear(Mat(H[8]), self.L8f, Mat(w['Y8']), 256, **kw)                 # feature vector -> Y8[:, 0:256]
-        linear(Mat(H[8]), self.L8s, Mat(w['Y8'], Y8_SDF), 1, **kw)          # sdf -> Y8[:, 260]
-        # reverse sweep for d sdf / d x  (v_k = sigma_k * u_{k+1}, u_k = W_k^T v_k)
+        H, V = w['H'], w['V']   # H[1..8]; H[4] has the PE/sqrt2 tail pre-filled by ray_fill
+        self.hidden_forward(w['X0'], H[1:], H[4], m_ptr, m_cap,
+                            heads=[CL(self.L8f, EK_BIAS_GENERIC, 256, save=Mat(w['Y8']), write_a=False),          # feature vector
+                                   CL(self.L8s, EK_BIAS_GENERIC, 1, save=Mat(w['Y8'], Y8_SDF), write_a=False)])   # sdf
+        # reverse sweep for d sdf / d x  (v_k = sigma_k * u_{k+1}, u_k = W_k^T v_k);
+        # u_4 = [217 -> v_3 (through 1/sqrt2) | 39 -> skip branch to the PE input]
         K('nero_dact_times_row', H[8], 256, self.L8s.w_eff, V[7], 256, 256, m_ptr, m_cap)
+        ls = []
         for k in range(7, 0, -1):
-            if k == 4:   # u_4 = [217 -> v_3 (through 1/sqrt2) | 39 -> skip branch to the PE input]
-                linear(Mat(V[4]), self.L[4], Mat(V[3]), 256, transposed=True, mode=EPI_MUL_DACT, oscale=INV_SQRT2, H=Mat(H[4]),
-                       hscale=SQRT2, dact=ACT_SOFTPLUS100, ncol_main=217, tail=Mat(w['USKIP']), **kw)
+            if k == 4:
+                ls.append(CL(self.L[4], EK_DACT_SOFTPLUS, 256, transposed=True, oscale=INV_SQRT2, H=Mat(H[4]), hscale=SQRT2,
+                             ncol_main=217, tail=Mat(w['USKIP']), save=Mat(V[3])))
             else:
-                linear(Mat(V[k]), self.L[k], Mat(V[k - 1]), 256, transposed=True, mode=EPI_MUL_DACT, H=Mat(H[k]),
-                       dact=ACT_SOFTPLUS100, **kw)
-        linear(Mat(V[0]), self.L[0], Mat(w['U0']), 39, transposed=True, mode=EPI_MUL_DACT, **kw)
+                ls.append(CL(self.L[k], EK_DACT_SOFTPLUS, 256, transposed=True, H=Mat(H[k]), save=Mat(V[k - 1])))
+        ls.append(CL(self.L[0], EK_DACT_NONE, 39, transposed=True, save=Mat(w['U0'])))
+        mlp(Mat(V[7]), ls, m_ptr, m_cap, tag='sdf_reverse_sweep', fused=USE_CHAIN)
         K('nero_pe_grad', w['X0'], 64, w['U0'], 64, w['USKIP'], 64, w['G'], m_ptr, m_cap)
 
     def backward(self, ws, w, m_ptr, m_cap, grads_of):
@@ -278,46 +227,25 @@ class SdfNet:
         # tangent sweep (adjoint of the reverse sweep): ubar_0 = J_PE dg ; vbar_k = W_k ubar_k ; ubar_{k+1} = sigma_k vbar_k,
         # which also leaves the softplus'' term q_k = 100 (1 - sigma_k) v_k vbar_k in ABAR[k]
         K('nero_pe_tangent', w['X0'], 64, w['DG'], UB[0], 64, UB[4], 256, m_ptr, m_cap)
-        if USE_CHAIN:
-            ls = []
-            for k in range(8):
-                if k == 3:
-                    ls.append(CL(self.L[3], EK_TANGENT, 217, use_bias=False, oscale=INV_SQRT2, H=Mat(H[4]), hscale=SQRT2, V=Mat(V[3]),
-                                 out2=Mat(AB[3]), save=Mat(UB[4]), csrc=Mat(UB[4])))
-                else:
-                    ls.append(CL(self.L[k], EK_TANGENT, 256, use_bias=False, H=Mat(H[k + 1]), V=Mat(V[k]), out2=Mat(AB[k]), save=Mat(UB[k + 1])))
-            chain(Mat(UB[0]), self.L[0].k_valid, ls, m_ptr, m_cap, tag='sdf_tangent_sweep')
-            # value backward: abar_7 = sigma_7*(W8f^T dfeat) + q_7 + dsdf*v_7 (v_7 = sigma_7*W8[0,:] from the reverse sweep);
-            # abar_{k-1} = sigma_{k-1} * (W_k^T abar_k) + q_{k-1}
-            K('nero_row_axpy', Mat(dY8, Y8_SDF), Y8_LD, V[7], 256, AB[7], 256, 256, m_ptr, m_cap)
-            ls = [CL(self.L8f, EK_DACT_SOFTPLUS, 256, transposed=True, H=Mat(H[8]), addend=Mat(AB[7]), save=Mat(AB[7]))]
-            for k in range(7, 0, -1):
-                if k == 4:
-                    ls.append(CL(self.L[4], EK_DACT_SOFTPLUS, 217, transposed=True, oscale=INV_SQRT2, H=Mat(H[4]), hscale=SQRT2,
-                                 addend=Mat(AB[3]), save=Mat(AB[3])))
-                else:
-                    ls.append(CL(self.L[k], EK_DACT_SOFTPLUS, 256, transposed=True, H=Mat(H[k]), addend=Mat(AB[k - 1]), save=Mat(AB[k - 1])))
-            chain(Mat(dY8), 256, ls, m_ptr, m_cap, tag='sdf_value_backward')
-        else:
-            for k in range(8):
-                A = Mat(UB[k])
-                if k == 3:
-                    linear(A, self.L[3], Mat(UB[4]), 217, use_bias=False, mode=EPI_TANGENT, oscale=INV_SQRT2, H=Mat(H[4]), hscale=SQRT2,
-                           dact=ACT_SOFTPLUS100, V=Mat(V[3]), out2=Mat(AB[3]), **kw)
-                else:
-                    linear(A, self.L[k], Mat(UB[k + 1]), 256, use_bias=False, mode=EPI_TANGENT, H=Mat(H[k + 1]), dact=ACT_SOFTPLUS100,
-                           V=Mat(V[k]), out2=Mat(AB[k]), **kw)
-            linear(Mat(dY8), self.L8f, Mat(AB[7]), 256, transposed=True, mode=EPI_MUL_DACT, H=Mat(H[8]), dact=ACT_SOFTPLUS100,
-                   addend=Mat(AB[7]), **kw)
-            linear(Mat(dY8, Y8_SDF), self.L8s, Mat(AB[7]), 256, transposed=True, mode=EPI_MUL_DACT, H=Mat(H[8]), dact=ACT_SOFTPLUS100,
-                   addend=Mat(AB[7]), **kw)
-            for k in range(7, 0, -1):
-                if k == 4:
-                    linear(Mat(AB[4]), self.L[4], Mat(AB[3]), 217, transposed=True, mode=EPI_MUL_DACT, oscale=INV_SQRT2, H=Mat(H[4]),
-                           hscale=SQRT2, dact=ACT_SOFTPLUS100, addend=Mat(AB[3]), **kw)
-                else:
-                    linear(Mat(AB[k]), self.L[k], Mat(AB[k - 1]), 256, transposed=True, mode=EPI_MUL_DACT, H=Mat(H[k]),
-                           dact=ACT_SOFTPLUS100, addend=Mat(AB[k - 1]), **kw)
+        ls = []
+        for k in range(8):
+            if k == 3:
+                ls.append(CL(self.L[3], EK_TANGENT, 217, use_bias=False, oscale=INV_SQRT2, H=Mat(H[4]), hscale=SQRT2, V=Mat(V[3]),
+                             out2=Mat(AB[3]), save=Mat(UB[4]), csrc=Mat(UB[4])))
+            else:
+                ls.append(CL(self.L[k], EK_TANGENT, 256, use_bias=False, H=Mat(H[k + 1]), V=Mat(V[k]), out2=Mat(AB[k]), save=Mat(UB[k + 1])))
+        mlp(Mat(UB[0]), ls, m_ptr, m_cap, tag='sdf_tangent_sweep', fused=USE_CHAIN)
+        # value backward: abar_7 = sigma_7*(W8f^T dfeat) + q_7 + dsdf*v_7 (v_7 = sigma_7*W8[0,:] from the reverse sweep);
+        # abar_{k-1} = sigma_{k-1} * (W_k^T abar_k) + q_{k-1}
+        K('nero_row_axpy', Mat(dY8, Y8_SDF), Y8_LD, V[7], 256, AB[7], 256, 256, m_ptr, m_cap)
+        ls = [CL(self.L8f, EK_DACT_SOFTPLUS, 256, transposed=True, H=Mat(H[8]), addend=Mat(AB[7]), save=Mat(AB[7]))]
+        for k in range(7, 0, -1):
+            if k == 4:
+                ls.append(CL(self.L[4], EK_DACT_SOFTPLUS, 217, transposed=True, oscale=INV_SQRT2, H=Mat(H[4]), hscale=SQRT2,
+                             addend=Mat(AB[3]), save=Mat(AB[3])))
+            else:
+                ls.append(CL(self.L[k], EK_DACT_SOFTPLUS, 256, transposed=True, H=Mat(H[k]), addend=Mat(AB[k - 1]), save=Mat(AB[k - 1])))
+        mlp(Mat(dY8), ls, m_ptr, m_cap, tag='sdf_value_backward', fused=USE_CHAIN)
         # weight gradients: dW_k = abar_k^T h_k + v_k^T ubar_k
         ls = self.sp.layers()
         for k in range(8):
@@ -337,12 +265,7 @@ class SdfNet:
 
     def value_forward(self, X0, H, out, m_ptr, m_cap):
         """SDF value with saved activations H[1..8] (step<1000 regulariser points, renderer.py:591-594)."""
-        Hs = [H[1], H[2], H[3], H[4], H[5], H[6], H[7], H[8]]
-        if USE_CHAIN:
-            self.hidden_forward(X0, Hs, H[4], m_ptr, m_cap, heads=[CL(self.L8s, EK_BIAS_GENERIC, 1, save=Mat(out), write_a=False)])
-        else:
-            self.hidden_forward(X0, Hs, H[4], m_ptr, m_cap)
-            linear(Mat(H[8]), self.L8s, Mat(out), 1, m_ptr=m_ptr, m_cap=m_cap)
+        self.hidden_forward(X0, H[1:], H[4], m_ptr, m_cap, heads=[CL(self.L8s, EK_BIAS_GENERIC, 1, save=Mat(out), write_a=False)])
 
     def value_backward(self, ws, X0, H, dsdf, AB, scratch, m_ptr, m_cap):
         """Backward of value_forward: dsdf [.,1] -> parameter grads.  abar_7 = dsdf * sigma_7 * W8[0,:], then the
@@ -357,16 +280,7 @@ class SdfNet:
                 ls.append(CL(self.L[4], EK_DACT_SOFTPLUS, 217, transposed=True, oscale=INV_SQRT2, H=Mat(H[4]), hscale=SQRT2, save=Mat(AB[3])))
             else:
                 ls.append(CL(self.L[k], EK_DACT_SOFTPLUS, 256, transposed=True, H=Mat(H[k]), save=Mat(AB[k - 1])))
-        if USE_CHAIN:
-            chain(Mat(AB[7]), 256, ls, m_ptr, m_cap)
-        else:
-            for k in range(7, 0, -1):
-                if k == 4:
-                    linear(Mat(AB[4]), self.L[4], Mat(AB[3]), 217, transposed=True, mode=EPI_MUL_DACT, oscale=INV_SQRT2, H=Mat(H[4]),
-                           hscale=SQRT2, dact=ACT_SOFTPLUS100, **kw)
-                else:
-                    linear(Mat(AB[k]), self.L[k], Mat(AB[k - 1]), 256, transposed=True, mode=EPI_MUL_DACT, H=Mat(H[k]),
-                           dact=ACT_SOFTPLUS100, **kw)
+        mlp(Mat(AB[7]), ls, m_ptr, m_cap, fused=USE_CHAIN)
         ls_ = self.sp.layers()
         for k in range(8):
             Hin = Mat(X0) if k == 0 else Mat(H[k])
@@ -406,35 +320,22 @@ class NerfNet:
     def forward(self, w, m_ptr, m_cap):
         kw = dict(m_ptr=m_ptr, m_cap=m_cap)
         N = w['NH']
-        if USE_CHAIN:
-            chain(Mat(w['XN']), self.P[0].k_valid,
-                  [CL(self.P[0], EK_BIAS_RELU, 256, save=Mat(N[1])), CL(self.P[1], EK_BIAS_RELU, 256, save=Mat(N[2])),
-                   CL(self.P[2], EK_BIAS_RELU, 256, save=Mat(N[3])), CL(self.P[3], EK_BIAS_RELU, 256, save=Mat(N[4])),
-                   CL(self.P[4], EK_BIAS_RELU, 256, save=Mat(w['H5'], 84), write_a=False)], m_ptr, m_cap, tag='nerf_fwd_a')
-            linear(Mat(w['H5']), self.P[5], Mat(N[6]), 256, act=ACT_RELU, **kw)     # K = 340 > 256: not chainable
-            chain(Mat(N[6]), 256,
-                  [CL(self.P[6], EK_BIAS_RELU, 256, save=Mat(N[7])), CL(self.P[7], EK_BIAS_RELU, 256, save=Mat(N[8])),
-                   CL(self.alpha, EK_BIAS_GENERIC, 1, save=Mat(w['DENS']), write_a=False),
-                   CL(self.feature, EK_BIAS_GENERIC, 256, save=Mat(w['FV']), write_a=False)], m_ptr, m_cap, tag='nerf_fwd_b')
-            linear(Mat(w['FV']), self.views, Mat(w['HV']), 128, act=ACT_RELU, **kw)
-            linear(Mat(w['HV']), self.rgb, Mat(w['RGBRAW']), 3, **kw)
-            return
-        linear(Mat(w['XN']), self.P[0], Mat(N[1]), 256, act=ACT_RELU, **kw)
-        linear(Mat(N[1]), self.P[1], Mat(N[2]), 256, act=ACT_RELU, **kw)
-        linear(Mat(N[2]), self.P[2], Mat(N[3]), 256, act=ACT_RELU, **kw)
-        linear(Mat(N[3]), self.P[3], Mat(N[4]), 256, act=ACT_RELU, **kw)
-        linear(Mat(N[4]), self.P[4], Mat(w['H5'], 84), 256, act=ACT_RELU, **kw)    # cat([input_pts, h]) (field.py:268-269)
-        linear(Mat(w['H5']), self.P[5], Mat(N[6]), 256, act=ACT_RELU, **kw)
-        linear(Mat(N[6]), self.P[6], Mat(N[7]), 256, act=ACT_RELU, **kw)
-        linear(Mat(N[7]), self.P[7], Mat(N[8]), 256, act=ACT_RELU, **kw)
-        linear(Mat(N[8]), self.alpha, Mat(w['DENS']), 1, **kw)
-        linear(Mat(N[8]), self.feature, Mat(w['FV']), 256, **kw)
+        mlp(Mat(w['XN']),
+            [CL(self.P[0], EK_BIAS_RELU, 256, save=Mat(N[1])), CL(self.P[1], EK_BIAS_RELU, 256, save=Mat(N[2])),
+             CL(self.P[2], EK_BIAS_RELU, 256, save=Mat(N[3])), CL(self.P[3], EK_BIAS_RELU, 256, save=Mat(N[4])),
+             CL(self.P[4], EK_BIAS_RELU, 256, save=Mat(w['H5'], 84), write_a=False)], m_ptr, m_cap, tag='nerf_fwd_a', fused=USE_CHAIN)
+        # layer 5 reads cat([input_pts, h]) (field.py:268-269): K = 340
+        mlp(Mat(w['H5']),
+            [CL(self.P[5], EK_BIAS_RELU, 256, save=Mat(N[6])), CL(self.P[6], EK_BIAS_RELU, 256, save=Mat(N[7])),
+             CL(self.P[7], EK_BIAS_RELU, 256, save=Mat(N[8])),
+             CL(self.alpha, EK_BIAS_GENERIC, 1, save=Mat(w['DENS']), write_a=False),
+             CL(self.feature, EK_BIAS_GENERIC, 256, save=Mat(w['FV']), write_a=False)], m_ptr, m_cap, tag='nerf_fwd_b', fused=USE_CHAIN)
         linear(Mat(w['FV']), self.views, Mat(w['HV']), 128, act=ACT_RELU, **kw)
         linear(Mat(w['HV']), self.rgb, Mat(w['RGBRAW']), 3, **kw)
 
     def backward(self, ws, w, m_ptr, m_cap):
         kw = dict(m_ptr=m_ptr, m_cap=m_cap)
-        N, dA, dB = w['NH'], w['dNa'], w['dNb']
+        N, dA, G = w['NH'], w['dNa'], w['dNG']   # G: pre-activation gradients of layers 6..0 (dA holds layer 7's)
         n = self.np
         gp = lambda l: (l.weight.grad, None, l.bias.grad)
         R = dict(transposed=True, mode=EPI_MUL_DACT, dact=ACT_RELU)
@@ -447,40 +348,22 @@ class NerfNet:
         wgrad(ws, Mat(w['dFV']), 256, Mat(N[8]), 256, self.feature, *gp(n.feature_linear), **kw)
         wgrad(ws, Mat(w['dDENS']), 1, Mat(N[8]), 256, self.alpha, *gp(n.alpha_linear), **kw)
         pl = n.pts_linears
-        if USE_CHAIN:
-            G = w['dNG']   # pre-activation gradients of layers 6..0 (dA holds layer 7's)
-            chain(Mat(dA), 256,
-                  [CL(self.P[7], EK_DACT_RELU, 256, transposed=True, H=Mat(N[7]), save=Mat(G[6])),
-                   CL(self.P[6], EK_DACT_RELU, 256, transposed=True, H=Mat(N[6]), save=Mat(G[5])),
-                   CL(self.P[5], EK_DACT_RELU, 256, transposed=True, H=Mat(w['H5'], 84), save=Mat(G[4])),
-                   CL(self.P[4], EK_DACT_RELU, 256, transposed=True, H=Mat(N[4]), save=Mat(G[3])),
-                   CL(self.P[3], EK_DACT_RELU, 256, transposed=True, H=Mat(N[3]), save=Mat(G[2])),
-                   CL(self.P[2], EK_DACT_RELU, 256, transposed=True, H=Mat(N[2]), save=Mat(G[1])),
-                   CL(self.P[1], EK_DACT_RELU, 256, transposed=True, H=Mat(N[1]), save=Mat(G[0]))], m_ptr, m_cap, tag='nerf_bwd')
-            wgrad(ws, Mat(dA), 256, Mat(N[7]), 256, self.P[7], *gp(pl[7]), **kw)
-            wgrad(ws, Mat(G[6]), 256, Mat(N[6]), 256, self.P[6], *gp(pl[6]), **kw)
-            wgrad(ws, Mat(G[5]), 256, Mat(w['H5']), self.P[5].k_valid, self.P[5], *gp(pl[5]), **kw)
-            wgrad(ws, Mat(G[4]), 256, Mat(N[4]), 256, self.P[4], *gp(pl[4]), **kw)
-            wgrad(ws, Mat(G[3]), 256, Mat(N[3]), 256, self.P[3], *gp(pl[3]), **kw)
-            wgrad(ws, Mat(G[2]), 256, Mat(N[2]), 256, self.P[2], *gp(pl[2]), **kw)
-            wgrad(ws, Mat(G[1]), 256, Mat(N[1]), 256, self.P[1], *gp(pl[1]), **kw)
-            wgrad(ws, Mat(G[0]), 256, Mat(w['XN']), self.P[0].k_valid, self.P[0], *gp(pl[0]), **kw)
-            return
-        linear(Mat(dA), self.P[7], Mat(dB), 256, H=Mat(N[7]), **R, **kw)
+        mlp(Mat(dA),
+            [CL(self.P[7], EK_DACT_RELU, 256, transposed=True, H=Mat(N[7]), save=Mat(G[6])),
+             CL(self.P[6], EK_DACT_RELU, 256, transposed=True, H=Mat(N[6]), save=Mat(G[5])),
+             CL(self.P[5], EK_DACT_RELU, 256, transposed=True, H=Mat(w['H5'], 84), save=Mat(G[4])),
+             CL(self.P[4], EK_DACT_RELU, 256, transposed=True, H=Mat(N[4]), save=Mat(G[3])),
+             CL(self.P[3], EK_DACT_RELU, 256, transposed=True, H=Mat(N[3]), save=Mat(G[2])),
+             CL(self.P[2], EK_DACT_RELU, 256, transposed=True, H=Mat(N[2]), save=Mat(G[1])),
+             CL(self.P[1], EK_DACT_RELU, 256, transposed=True, H=Mat(N[1]), save=Mat(G[0]))], m_ptr, m_cap, tag='nerf_bwd', fused=USE_CHAIN)
         wgrad(ws, Mat(dA), 256, Mat(N[7]), 256, self.P[7], *gp(pl[7]), **kw)
-        linear(Mat(dB), self.P[6], Mat(dA), 256, H=Mat(N[6]), **R, **kw)
-        wgrad(ws, Mat(dB), 256, Mat(N[6]), 256, self.P[6], *gp(pl[6]), **kw)
-        linear(Mat(dA), self.P[5], Mat(dB), 256, H=Mat(w['H5'], 84), **R, **kw)
-        wgrad(ws, Mat(dA), 256, Mat(w['H5']), self.P[5].k_valid, self.P[5], *gp(pl[5]), **kw)
-        linear(Mat(dB), self.P[4], Mat(dA), 256, H=Mat(N[4]), **R, **kw)
-        wgrad(ws, Mat(dB), 256, Mat(N[4]), 256, self.P[4], *gp(pl[4]), **kw)
-        linear(Mat(dA), self.P[3], Mat(dB), 256, H=Mat(N[3]), **R, **kw)
-        wgrad(ws, Mat(dA), 256, Mat(N[3]), 256, self.P[3], *gp(pl[3]), **kw)
-        linear(Mat(dB), self.P[2], Mat(dA), 256, H=Mat(N[2]), **R, **kw)
-        wgrad(ws, Mat(dB), 256, Mat(N[2]), 256, self.P[2], *gp(pl[2]), **kw)
-        linear(Mat(dA), self.P[1], Mat(dB), 256, H=Mat(N[1]), **R, **kw)
-        wgrad(ws, Mat(dA), 256, Mat(N[1]), 256, self.P[1], *gp(pl[1]), **kw)
-        wgrad(ws, Mat(dB), 256, Mat(w['XN']), self.P[0].k_valid, self.P[0], *gp(pl[0]), **kw)
+        wgrad(ws, Mat(G[6]), 256, Mat(N[6]), 256, self.P[6], *gp(pl[6]), **kw)
+        wgrad(ws, Mat(G[5]), 256, Mat(w['H5']), self.P[5].k_valid, self.P[5], *gp(pl[5]), **kw)
+        wgrad(ws, Mat(G[4]), 256, Mat(N[4]), 256, self.P[4], *gp(pl[4]), **kw)
+        wgrad(ws, Mat(G[3]), 256, Mat(N[3]), 256, self.P[3], *gp(pl[3]), **kw)
+        wgrad(ws, Mat(G[2]), 256, Mat(N[2]), 256, self.P[2], *gp(pl[2]), **kw)
+        wgrad(ws, Mat(G[1]), 256, Mat(N[1]), 256, self.P[1], *gp(pl[1]), **kw)
+        wgrad(ws, Mat(G[0]), 256, Mat(w['XN']), self.P[0].k_valid, self.P[0], *gp(pl[0]), **kw)
 
 
 class ShapeEngine:
@@ -627,7 +510,7 @@ class ShapeEngine:
         w['UB'] = [z(cap, 64)] + [z(cap, 256) for _ in range(8)]
         w['ABAR'] = [z(cap, 256) for _ in range(8)]
         w.update(dALPHA_OUT=z(cap), dCOLOR_OUT=z(cap, 4), dDENS=z(cap, 4), dRGBRAW=z(cap, 4), dHV=z(cap, 128), dFV=z(cap, 256),
-                 dNa=z(cap, 256), dNb=z(cap, 256))
+                 dNa=z(cap, 256))
         w['dNG'] = [z(cap, 256) for _ in range(7)]
         self.bw_ready = True
 
@@ -934,20 +817,20 @@ class ShapeEngine:
         K('nero_shade_combine_bwd', w['OUTS'], w['GEO'], self.lut, self.exp_max, 1 if self.human else 0, w['dCOLOR_IN'], docc, w['DOUTS'],
           w['DNOV'], n_in, cap)
         A = w['ACT']
-        dHa, dHb, dHc = w['dHa'], w['dHb'], w['dHc']
+        dH = (w['dHa'], w['dHb'], w['dHc'])
         ko = 144 if self.sphere else 72
-        self.m_outer.backward(ws, Mat(w['DOUTS'], O_LDIR), Mat(w['E'], E_IDER), A['odir'], dHa, dHb, n_in, cap, dX=Mat(w['dE_dir']), dx_ncol=ko, dHc=dHc)
-        self.m_outer.backward(ws, Mat(w['DOUTS'], O_LD), Mat(w['E'], self.e_iden), A['odif'], dHa, dHb, n_in, cap, dX=Mat(w['dE_dif']), dx_ncol=ko, dHc=dHc)
-        self.m_inner.backward(ws, Mat(w['DOUTS'], O_LI), Mat(w['E'], E_PE8X), A['inner'], dHa, dHb, n_in, cap, dX=Mat(w['dE_inn']), dx_ncol=72, dHc=dHc)
-        self.m_iw.backward(ws, Mat(w['DOUTS'], O_IW), Mat(w['E'], 0), A['iw'], dHa, dHb, n_in, cap, dHc=dHc)
+        self.m_outer.backward(ws, Mat(w['DOUTS'], O_LDIR), Mat(w['E'], E_IDER), A['odir'], dH, n_in, cap, dX=Mat(w['dE_dir']), dx_ncol=ko)
+        self.m_outer.backward(ws, Mat(w['DOUTS'], O_LD), Mat(w['E'], self.e_iden), A['odif'], dH, n_in, cap, dX=Mat(w['dE_dif']), dx_ncol=ko)
+        self.m_inner.backward(ws, Mat(w['DOUTS'], O_LI), Mat(w['E'], E_PE8X), A['inner'], dH, n_in, cap, dX=Mat(w['dE_inn']), dx_ncol=72)
+        self.m_iw.backward(ws, Mat(w['DOUTS'], O_IW), Mat(w['E'], 0), A['iw'], dH, n_in, cap)
         if self.human:
-            self.m_human.backward(ws, Mat(w['DOUTS'], O_HUM), Mat(w['EH']), A['human'], dHa, dHb, n_in, cap, dX=Mat(w['dEH']), dx_ncol=24, dHc=dHc)
+            self.m_human.backward(ws, Mat(w['DOUTS'], O_HUM), Mat(w['EH']), A['human'], dH, n_in, cap, dX=Mat(w['dEH']), dx_ncol=24)
         K('nero_shade_prep_bwd', w['G'], w['PTS'], w['RAY_IN'], rays_d, w['OUTS'], w['GEO'], w['dE_dir'], 160, w['dE_inn'], 128, w['dE_dif'], 160,
           w['dEH'] if self.human else None, 64, st['hp'], w['DNOV'], w['DOUTS'], w['DG'], n_in, cap, 1 if self.sphere else 0)
         matin = Mat(w['Y8'])
-        self.m_rough.backward(ws, Mat(w['DOUTS'], O_ROUGH), matin, A['rough'], dHa, dHb, n_in, cap, dX=Mat(w['dY8']), dx_ncol=256, dHc=dHc)
-        self.m_met.backward(ws, Mat(w['DOUTS'], O_MET), matin, A['met'], dHa, dHb, n_in, cap, dX=Mat(w['dY8']), dx_ncol=256, dx_addend=Mat(w['dY8']), dHc=dHc)
-        self.m_alb.backward(ws, Mat(w['DOUTS'], O_ALB), matin, A['alb'], dHa, dHb, n_in, cap, dX=Mat(w['dY8']), dx_ncol=256, dx_addend=Mat(w['dY8']), dHc=dHc)
+        self.m_rough.backward(ws, Mat(w['DOUTS'], O_ROUGH), matin, A['rough'], dH, n_in, cap, dX=Mat(w['dY8']), dx_ncol=256)
+        self.m_met.backward(ws, Mat(w['DOUTS'], O_MET), matin, A['met'], dH, n_in, cap, dX=Mat(w['dY8']), dx_ncol=256, dx_addend=Mat(w['dY8']))
+        self.m_alb.backward(ws, Mat(w['DOUTS'], O_ALB), matin, A['alb'], dH, n_in, cap, dX=Mat(w['dY8']), dx_ncol=256, dx_addend=Mat(w['dY8']))
         # ---- SDF -> alpha
         w['D_INV_S'].zero_()
         dg = None if d_gerr is None else d_gerr.contiguous()

@@ -18,7 +18,8 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import ops
-from .ops import Mat, K, linear, wgrad, chain, chain_layer as CL, ACT_RELU, ACT_SIGMOID, ACT_EXPCLAMP
+# linear is not called here (see the note on chain in engine.py): it stays bound for the GEMM census
+from .ops import Mat, K, linear, wgrad, chain, mlp, chain_layer as CL, ACT_SIGMOID, ACT_EXPCLAMP
 from .ops import EK_BIAS_RELU, EK_BIAS_GENERIC, EK_DACT_RELU
 from .engine import Predictor, Grads, upload_ide_table, _linear_to_srgb_torch
 from .params import MCShadingParams
@@ -93,14 +94,15 @@ class FeatsNet:
 
     def forward(self, w, M):
         A, B = w['FA'], w['FB']
-        chain(Mat(w['FX']), self.L0[0].k_valid,
-              [CL(self.L0[0], EK_BIAS_RELU, 256, save=Mat(A[0])), CL(self.L0[1], EK_BIAS_RELU, 256, save=Mat(A[1])),
-               CL(self.L0[2], EK_BIAS_RELU, 256, save=Mat(A[2])),
-               CL(self.L0[3], EK_BIAS_RELU, 256, save=Mat(w['FCAT']), write_a=False)], None, M, tag='feats_a')
-        linear(Mat(w['FCAT']), self.L1[0], Mat(B[0]), 256, act=ACT_RELU, m_cap=M)       # K = 307 > 256: not chainable
-        chain(Mat(B[0]), 256,
-              [CL(self.L1[1], EK_BIAS_RELU, 256, save=Mat(B[1])), CL(self.L1[2], EK_BIAS_RELU, 256, save=Mat(B[2])),
-               CL(self.L1[3], EK_BIAS_GENERIC, 256, save=Mat(w['FY']), write_a=False)], None, M, tag='feats_b')
+        mlp(Mat(w['FX']),
+            [CL(self.L0[0], EK_BIAS_RELU, 256, save=Mat(A[0])), CL(self.L0[1], EK_BIAS_RELU, 256, save=Mat(A[1])),
+             CL(self.L0[2], EK_BIAS_RELU, 256, save=Mat(A[2])),
+             CL(self.L0[3], EK_BIAS_RELU, 256, save=Mat(w['FCAT']), write_a=False)], None, M, tag='feats_a')
+        # the second half reads cat([h, PE8]): K = 307
+        mlp(Mat(w['FCAT']),
+            [CL(self.L1[0], EK_BIAS_RELU, 256, save=Mat(B[0])), CL(self.L1[1], EK_BIAS_RELU, 256, save=Mat(B[1])),
+             CL(self.L1[2], EK_BIAS_RELU, 256, save=Mat(B[2])),
+             CL(self.L1[3], EK_BIAS_GENERIC, 256, save=Mat(w['FY']), write_a=False)], None, M, tag='feats_b')
 
     def backward(self, ws, w, M):
         """w['dFY'][:, :256] holds d(feats); accumulates all 8 layers' parameter gradients."""
@@ -224,11 +226,11 @@ class MaterialEngine:
         d[:, O_ROUGH:O_ROUGH + 1] = sg(o[:, O_ROUGH:O_ROUGH + 1], d_rough)
         d[:, O_ALB:O_ALB + 3] = sg(o[:, O_ALB:O_ALB + 3], d_alb)
         y, dy = Mat(w['FY']), Mat(w['dFY'])
-        a = (w['dHa'], w['dHb'])
+        dH = (w['dHa'], w['dHb'], w['dHc'])
         dm = w['DOUT']
-        self.m_rough.backward(self.ws, Mat(dm, O_ROUGH), y, w['ACT']['rough'], *a, None, M, dX=dy, dx_ncol=256, dHc=w['dHc'])
-        self.m_met.backward(self.ws, Mat(dm, O_MET), y, w['ACT']['met'], *a, None, M, dX=dy, dx_ncol=256, dx_addend=dy, dHc=w['dHc'])
-        self.m_alb.backward(self.ws, Mat(dm, O_ALB), y, w['ACT']['alb'], *a, None, M, dX=dy, dx_ncol=256, dx_addend=dy, dHc=w['dHc'])
+        self.m_rough.backward(self.ws, Mat(dm, O_ROUGH), y, w['ACT']['rough'], dH, None, M, dX=dy, dx_ncol=256)
+        self.m_met.backward(self.ws, Mat(dm, O_MET), y, w['ACT']['met'], dH, None, M, dX=dy, dx_ncol=256, dx_addend=dy)
+        self.m_alb.backward(self.ws, Mat(dm, O_ALB), y, w['ACT']['alb'], dH, None, M, dX=dy, dx_ncol=256, dx_addend=dy)
         self.feats.backward(self.ws, w, M)
         self.ws.flush()
 
@@ -318,14 +320,14 @@ class MaterialEngine:
         A, D = w['ACT'], w['dH']
         if n_miss > 0:
             ko = 144 if self.sphere else 72
-            self.m_outer.backward(self.ws, Mat(w['DPRE_O']), Mat(w['EO']), [a[:n_miss] for a in A], D[0][:n_miss], D[1][:n_miss], None, n_miss,
-                                  dX=Mat(w['dEO']), dx_ncol=ko, dHc=D[2][:n_miss])
+            self.m_outer.backward(self.ws, Mat(w['DPRE_O']), Mat(w['EO']), [a[:n_miss] for a in A], [d[:n_miss] for d in D], None, n_miss,
+                                  dX=Mat(w['dEO']), dx_ncol=ko)
             if self.human:
-                self.m_human.backward(self.ws, Mat(w['DPRE_H']), Mat(w['EH']), w['ACTH'], D[0][:n_miss], D[1][:n_miss], None, n_miss,
-                                      dX=Mat(w['dEH']), dx_ncol=24, dHc=D[2][:n_miss])
+                self.m_human.backward(self.ws, Mat(w['DPRE_H']), Mat(w['EH']), w['ACTH'], [d[:n_miss] for d in D], None, n_miss,
+                                      dX=Mat(w['dEH']), dx_ncol=24)
         if n_hit > 0:
-            self.m_inner.backward(self.ws, Mat(w['DPRE_I']), Mat(w['EI']), [a[n_miss:] for a in A], D[0][n_miss:], D[1][n_miss:], None, n_hit,
-                                  dX=Mat(w['dEI'], 52), dx_ncol=72, dHc=D[2][n_miss:])
+            self.m_inner.backward(self.ws, Mat(w['DPRE_I']), Mat(w['EI']), [a[n_miss:] for a in A], [d[n_miss:] for d in D], None, n_hit,
+                                  dX=Mat(w['dEI'], 52), dx_ncol=72)
         self.ws.flush()
         K('nero_mc_dir_bwd', q)
         return w['dA'][:st['P']] + w['dA2'][:st['P']]

@@ -209,6 +209,13 @@ class PreparedLayer:
     def bias_view(self):
         return None if self.bias is None else self.bias.detach()[self.row0:self.row0 + self.nrows]
 
+    def operand(self, transposed, use_bias=True):
+        """(image, n_pad, k_chunks, k_valid, bias) of a GEMM through this layer: forward (out = A W^T + b over the layout
+        columns) or transposed (out = A W restricted to t_cols, contracting over the nrows outputs, no bias)."""
+        if transposed:
+            return self.img_t, self.t_npad, self.t_chunks, ceil_div(self.nrows, 4) * 4, None
+        return self.img_f, self.n_pad, self.k_chunks, self.k_valid, self.bias_view() if use_bias else None
+
 
 class PrepBatch:
     """PreparedLayer.prep() of many layers as ONE nero_prep_weight_batch launch.  The job table only holds device pointers;
@@ -261,12 +268,7 @@ def linear(A: Mat, layer: PreparedLayer, out: Mat, ncol_out, *, transposed=False
     """out = epilogue(A @ W^T) (transposed=False) or epilogue(A @ W) restricted to t_cols (transposed=True)."""
     if ncol_main is None:
         ncol_main = ncol_out
-    if transposed:
-        img, n_pad, k_chunks, k_valid = layer.img_t, layer.t_npad, layer.t_chunks, ceil_div(layer.nrows, 4) * 4
-        bias = None
-    else:
-        img, n_pad, k_chunks, k_valid = layer.img_f, layer.n_pad, layer.k_chunks, layer.k_valid
-        bias = layer.bias_view() if use_bias else None
+    img, n_pad, k_chunks, k_valid, bias = layer.operand(transposed, use_bias)
     if m_cap is None:
         m_cap = A.t.shape[0]
     K('nero_linear', A, A.ld, k_valid, img, n_pad, k_chunks, bias, 0 if bias is None else bias.numel(), out, out.ld, ncol_out,
@@ -401,11 +403,13 @@ EK_BIAS_SOFTPLUS, EK_BIAS_RELU, EK_BIAS_GENERIC, EK_DACT_SOFTPLUS, EK_DACT_RELU,
 
 def chain_layer(layer: PreparedLayer, kind, ncol_out, *, transposed=False, save: Mat = None, act=ACT_NONE, act_param=0.0, oscale=1.0,
                 H: Mat = None, hscale=1.0, V: Mat = None, out2: Mat = None, addend: Mat = None, ncol_main=None, tail: Mat = None,
-                write_a=True, csrc: Mat = None, use_bias=True):
-    """Describe one layer of a fused chain (same semantics as ops.linear for the matching kind)."""
+                write_a=True, csrc: Mat = None, use_bias=True, store=True):
+    """Describe one layer of a fused chain (same semantics as ops.linear for the matching kind).  store=False (read by
+    mlp()): the fused chain gets no `save` and keeps the output in shared memory only; the per-layer expansion still writes
+    `save`, because its next launch reads the output from there."""
     return dict(layer=layer, kind=kind, ncol_out=ncol_out, transposed=transposed, save=save, act=act, act_param=act_param, oscale=oscale,
                 H=H, hscale=hscale, V=V, out2=out2, addend=addend, ncol_main=ncol_out if ncol_main is None else ncol_main, tail=tail,
-                write_a=write_a, csrc=csrc, use_bias=use_bias)
+                write_a=write_a, csrc=csrc, use_bias=use_bias, store=store)
 
 
 PROFILE = None   # bench.py: list collecting (tag, event0, event1, flops_per_row, m_ptr_addr, m_cap) per chain launch
@@ -421,16 +425,11 @@ def chain(A0: Mat, k_valid0, layers, m_ptr=None, m_cap=None, tag=''):
     P.A0, P.lda0, P.k_valid0 = _addr(A0), A0.ld, ceil_div(k_valid0, 4) * 4
     P.n_layers, P.m_ptr, P.m_cap = len(layers), _addr(m_ptr), m_cap
     P.phase_clk = _addr(CHAIN_PHASES)
-    keep = []
+    opnd = [d['layer'].operand(d['transposed'], d['use_bias']) for d in layers]
     for i, d in enumerate(layers):
-        lay, L = d['layer'], P.L[i]
-        if d['transposed']:
-            img, n_pad, k_chunks, bias = lay.img_t, lay.t_npad, lay.t_chunks, None
-        else:
-            img, n_pad, k_chunks = lay.img_f, lay.n_pad, lay.k_chunks
-            bias = lay.bias_view() if d['use_bias'] else None
+        L = P.L[i]
+        img, n_pad, k_chunks, _, bias = opnd[i]
         assert k_chunks <= 4 and d['ncol_out'] <= n_pad
-        keep.append(bias)
         L.wimg, L.bias, L.n_bias = _addr(img), _addr(bias), 0 if bias is None else bias.numel()
         L.n_pad, L.k_chunks, L.ncol_out, L.ncol_main, L.kind, L.act = n_pad, k_chunks, d['ncol_out'], d['ncol_main'], d['kind'], d['act']
         for name, ldname in (('save', 'ld_save'), ('H', 'ldh'), ('addend', 'ldadd'), ('V', 'ldv'), ('out2', 'ldo2'), ('tail', 'ldt'),
@@ -440,10 +439,8 @@ def chain(A0: Mat, k_valid0, layers, m_ptr=None, m_cap=None, tag=''):
             setattr(L, ldname, m.ld if m is not None else 0)
         L.oscale, L.hscale, L.act_param = d['oscale'], d['hscale'], d['act_param']
         L.write_a = 1 if (d['write_a'] and i + 1 < len(layers)) else 0
-        nxt = layers[i + 1]['layer'] if i + 1 < len(layers) else None
-        if nxt is not None:
-            nk = nxt.t_chunks if layers[i + 1]['transposed'] else nxt.k_chunks
-            L.a_blocks = 4 * nk
+        if i + 1 < len(layers):
+            L.a_blocks = 4 * opnd[i + 1][2]
     if PROFILE is not None:
         fl = 0.0
         for d in layers:
@@ -456,6 +453,37 @@ def chain(A0: Mat, k_valid0, layers, m_ptr=None, m_cap=None, tag=''):
     if PROFILE is not None:
         e1.record()
         PROFILE.append((tag, e0, e1, fl, None if m_ptr is None else m_ptr.data_ptr(), m_cap))
+
+
+# chain kind -> the nero_linear (mode, act, dact) with the same epilogue; act None: the descriptor's own act
+_LINEAR_EPILOGUE = {EK_BIAS_SOFTPLUS: (EPI_BIAS_ACT, ACT_SOFTPLUS100, ACT_NONE), EK_BIAS_RELU: (EPI_BIAS_ACT, ACT_RELU, ACT_NONE),
+                    EK_BIAS_GENERIC: (EPI_BIAS_ACT, None, ACT_NONE), EK_DACT_SOFTPLUS: (EPI_MUL_DACT, ACT_NONE, ACT_SOFTPLUS100),
+                    EK_DACT_RELU: (EPI_MUL_DACT, ACT_NONE, ACT_RELU), EK_DACT_NONE: (EPI_MUL_DACT, ACT_NONE, ACT_NONE),
+                    EK_TANGENT: (EPI_TANGENT, ACT_NONE, ACT_SOFTPLUS100)}
+
+
+def mlp(A0: Mat, layers, m_ptr=None, m_cap=None, tag='', fused=True):
+    """Run a pass stated as chain_layer descriptors; A0 holds the first layer's input.
+
+    fused: the leading layers whose operand has more than 4 K chunks (K > 256 does not fit the chain's shared-memory A
+    operand) run as nero_linear, the rest as one nero_chain.  Otherwise every layer is one nero_linear launch with the same
+    epilogue, so the per-layer path runs exactly the layers of the fused one.  The next layer reads the output a layer
+    saves when it has write_a, else the same A (the heads)."""
+    A = A0
+    for i, d in enumerate(layers):
+        _, _, k_chunks, k_valid, _ = d['layer'].operand(d['transposed'], False)
+        if fused and k_chunks <= 4:
+            chain(A, k_valid, [d if d['store'] else dict(d, save=None) for d in layers[i:]], m_ptr, m_cap, tag)
+            return
+        mode, act, dact = _LINEAR_EPILOGUE[d['kind']]
+        save = d['save']
+        linear(A, d['layer'], save, d['ncol_out'], transposed=d['transposed'], mode=mode, act=d['act'] if act is None else act,
+               act_param=d['act_param'], oscale=d['oscale'], H=d['H'], hscale=d['hscale'], dact=dact, V=d['V'], out2=d['out2'],
+               addend=d['addend'], ncol_main=d['ncol_main'], tail=d['tail'], m_ptr=m_ptr, m_cap=m_cap, use_bias=d['use_bias'])
+        # a skip-concat's extra columns are already in the saved output's buffer: the next layer reads them from there
+        assert d['csrc'] is None or (d['csrc'].t is save.t and d['csrc'].c0 == save.c0)
+        if d['write_a']:
+            A = Mat(save.t, save.c0)
 
 
 # ------------------------------------------------------------------------------------------------ stage II (k_bvh.cu)

@@ -6,12 +6,15 @@ The product package has no alternate backend; this harness substitutes things fr
     (count, then each argtype's from_param), so the walk checks the signature of every call site it reaches; the few entry
     points whose device-side counts drive host control flow write plausible counts through the (CPU) pointers they were given;
   * `ops._stream` returns a null stream, `ops.require_cuda` accepts any device;
-  * `ops.linear / chain / wgrad` are wrapped with the argument / buffer-shape assertions a wrong call sequence would trip.
+  * `ops.linear / chain / wgrad` are wrapped with the argument / buffer-shape assertions a wrong call sequence would trip,
+    and every GEMM layer they launch is appended to GEMMS.
 Numerical results are meaningless in this mode.
 """
 import ctypes
 
 from nero_b200 import ops
+
+GEMMS = []    # (PreparedLayer, transposed, ncol_out) of every nero_linear launch and every nero_chain layer, in launch order
 
 
 class FakeLib:
@@ -86,8 +89,8 @@ def install():
     real_linear, real_chain, real_wgrad = ops.linear, ops.chain, ops.wgrad
 
     def linear(A, layer, out, ncol_out, *, transposed=False, mode=ops.EPI_BIAS_ACT, H=None, V=None, out2=None, **kw):
-        img, n_pad = (layer.img_t, layer.t_npad) if transposed else (layer.img_f, layer.n_pad)
-        k_valid = ops.ceil_div(layer.nrows, 4) * 4 if transposed else layer.k_valid
+        img, n_pad, _, k_valid, _ = layer.operand(transposed, False)
+        GEMMS.append((layer, transposed, ncol_out))
         assert A.ld % 4 == 0 and A.c0 % 4 == 0 and ncol_out <= n_pad and img is not None
         assert A.c0 + k_valid <= A.t.shape[1] and out.c0 + ncol_out <= out.t.shape[1], (A.c0, k_valid, A.t.shape, out.c0, ncol_out, out.t.shape)
         assert mode != ops.EPI_TANGENT or (H is not None and V is not None and out2 is not None)
@@ -97,7 +100,8 @@ def install():
         assert A0.c0 % 4 == 0 and A0.ld % 4 == 0 and A0.c0 + ops.ceil_div(k_valid0, 4) * 4 <= A0.t.shape[1]
         for d in layers:
             lay = d['layer']
-            assert (lay.img_t if d['transposed'] else lay.img_f) is not None
+            GEMMS.append((lay, d['transposed'], d['ncol_out']))
+            assert lay.operand(d['transposed'], False)[0] is not None
             if d['kind'] in (ops.EK_DACT_SOFTPLUS, ops.EK_DACT_RELU, ops.EK_TANGENT):
                 assert d['H'] is not None
             if d['kind'] == ops.EK_TANGENT:

@@ -44,6 +44,38 @@ SCRIPT = textwrap.dedent('''
     assert net.nvs(pose, K, 8, 12).shape == (8, 12, 3)
     assert net.sdf_network.sdf(torch.zeros(5, 7, 3)).shape == (5, 7, 1)
 
+    # ---- the per-layer path (USE_CHAIN = False) runs the GEMM layers of the fused chains, in the same order
+    import nero_b200.engine as E
+    net = NeROShapeRenderer({'n_samples': 32, 'n_importance': 32}, training=False)
+
+    def train(step):
+        net.zero_grad()
+        out = net.render(r['rays_o'], r['rays_d'], r['near'], r['far'], r['human_poses'], -1, net.get_anneal_val(step), True, step)
+        loss = torch.mean(net.compute_rgb_loss(out['ray_rgb'], r['rgb'])) + torch.mean(out['gradient_error']) + torch.mean(out['loss_occ'])
+        (loss + out['sdf_vals'].sum() * 0 if step < 1000 else loss).backward()
+
+    def validation():
+        with torch.no_grad():
+            net.render(r['rays_o'], r['rays_d'], r['near'], r['far'], r['human_poses'], 0, 0, False, 30000)
+    walks = {'step 500': lambda: train(500), 'step 30000': lambda: train(30000), 'validation render': validation,
+             'materials_query': lambda: net.predict_materials(torch.rand(40, 3), batch_size=16),
+             'sdf_query': lambda: net.sdf_network.sdf(torch.rand(5, 7, 3))}
+    show = lambda g: (g[0].nrows, g[0].K, 'transposed' if g[1] else 'forward', g[2])
+    differ = []
+    for name, walk in walks.items():
+        seqs = []
+        for fused in (True, False):
+            E.USE_CHAIN = fused
+            dry_run_harness.GEMMS.clear()
+            walk()
+            seqs.append(list(dry_run_harness.GEMMS))     # (PreparedLayer, transposed, ncol_out); layers compare by identity
+        if seqs[0] != seqs[1]:
+            i = next((i for i, (a, b) in enumerate(zip(*seqs)) if a != b), min(map(len, seqs)))
+            differ.append(f'{name}: {len(seqs[0])} fused / {len(seqs[1])} per-layer GEMM layers, first difference at #{i}: '
+                          f'{[show(s[i]) if i < len(s) else None for s in seqs]}')
+    E.USE_CHAIN = True
+    assert not differ, differ
+
     # ---- stage II: train step (all shader variants), ray-batch construction through the tracer, image chunk loop
     verts, tris = OM.test_scene(1)
     for scfg in ({'human_lights': False}, {'human_lights': True, 'outer_light_version': 'sphere_direction', 'geometry_type': 'ggx_smith'}):

@@ -40,6 +40,9 @@ MAX_MSGS = 12
 
 def _caller(depth):
     f = sys._getframe(depth + 1)
+    from nero_b200 import ops
+    if f.f_code is ops.mlp.__code__:      # name the line that states the pass, not the runner's launch
+        f = f.f_back
     return f'{os.path.basename(f.f_code.co_filename)}:{f.f_lineno}'
 
 

@@ -159,11 +159,12 @@ def test_wgrad_device_row_count_masks_stale_rows():
 
 @pytest.mark.parametrize('M', [3000, 45001])
 def test_chain_matches_layerwise_and_fp64(M):
-    """Fused chain (A operand in shared memory) vs fp64 torch: 3 softplus layers with the skip-concat, then a linear head;
-    then a derivative (DACT) chain in the reverse direction with addend / tail.  M = 45001 is 352 row tiles: every one of
-    the 132 persistent CTAs loops over at least two tiles (mbarrier phases across tiles) and the last tile is ragged."""
+    """Fused chain (A operand in shared memory) and its one-nero_linear-per-layer expansion (ops.mlp) vs fp64 torch:
+    3 softplus layers with the skip-concat, then a linear head; then a derivative (DACT) chain in the reverse direction with
+    addend / tail.  M = 45001 is 352 row tiles: every one of the 132 persistent CTAs loops over at least two tiles (mbarrier
+    phases across tiles) and the last tile is ragged."""
     from nero_b200 import ops
-    from nero_b200.ops import Mat, chain, chain_layer as CL
+    from nero_b200.ops import Mat, mlp, chain_layer as CL
     dev = torch.device('cuda')
     L0, W0, b0 = _mk_layer(ops, 256, 39, dev, seed=1, t_cols=(0, 39))
     L1, W1, b1 = _mk_layer(ops, 217, 256, dev, seed=2, t_cols=(0, 256))
@@ -172,42 +173,48 @@ def test_chain_matches_layerwise_and_fp64(M):
     X = torch.zeros(M, 64, device=dev)
     X[:, :39] = torch.randn(M, 39, device=dev) * 0.5
     H1, H2, H3 = torch.zeros(M, 256, device=dev), torch.zeros(M, 256, device=dev), torch.zeros(M, 256, device=dev)
-    H2[:, 217:] = X[:, :39] * 0.5                     # concat source pre-filled in the save buffer
     out = torch.zeros(M, 32, device=dev)
-    chain(Mat(X), 40, [CL(L0, ops.EK_BIAS_SOFTPLUS, 256, save=Mat(H1)),
-                       CL(L1, ops.EK_BIAS_SOFTPLUS, 217, oscale=0.70710678, save=Mat(H2), csrc=Mat(H2)),
-                       CL(L2, ops.EK_BIAS_SOFTPLUS, 256, save=Mat(H3)),
-                       CL(L3, ops.EK_BIAS_GENERIC, 3, act=3, save=Mat(out, 8), write_a=False)])
-    torch.cuda.synchronize()
     sp = lambda x: torch.nn.functional.softplus(x, beta=100)
     h1 = sp(X[:, :39].double() @ W0.t() + b0)
     h2 = torch.cat([0.70710678 * sp(h1 @ W1.t() + b1), X[:, :39].double() * 0.5], -1)
     h3 = sp(h2 @ W2.t() + b2)
     o = torch.sigmoid(h3 @ W3.t() + b3)
-    for nm, got, want in [('h1', H1, h1), ('h2', H2, h2), ('h3', H3, h3), ('out', out[:, 8:11], o)]:
-        e = float((got.double() - want).abs().max())
-        print(f'chain fwd {nm}: max abs err {e:.2e} (|want| max {float(want.abs().max()):.2e})')
-        assert e < 3e-5 * max(1.0, float(want.abs().max()))
+    for fused in (True, False):
+        for t in (H1, H2, H3, out):
+            t.zero_()
+        H2[:, 217:] = X[:, :39] * 0.5                 # concat source pre-filled in the save buffer
+        mlp(Mat(X), [CL(L0, ops.EK_BIAS_SOFTPLUS, 256, save=Mat(H1)),
+                     CL(L1, ops.EK_BIAS_SOFTPLUS, 217, oscale=0.70710678, save=Mat(H2), csrc=Mat(H2)),
+                     CL(L2, ops.EK_BIAS_SOFTPLUS, 256, save=Mat(H3)),
+                     CL(L3, ops.EK_BIAS_GENERIC, 3, act=3, save=Mat(out, 8), write_a=False)], fused=fused)
+        torch.cuda.synchronize()
+        for nm, got, want in [('h1', H1, h1), ('h2', H2, h2), ('h3', H3, h3), ('out', out[:, 8:11], o)]:
+            e = float((got.double() - want).abs().max())
+            print(f'{"chain" if fused else "layerwise"} fwd {nm}: max abs err {e:.2e} (|want| max {float(want.abs().max()):.2e})')
+            assert e < 3e-5 * max(1.0, float(want.abs().max()))
     # derivative chain: g2 = dact(H3) * (G @ W2) [217 main + tail], g1 = dact(H2*sqrt2)*... , g0 = g1 @ W0 (no dact)
     G = torch.randn(M, 256, device=dev)
     V2, V1, U0, TL = torch.zeros(M, 256, device=dev), torch.zeros(M, 256, device=dev), torch.zeros(M, 64, device=dev), torch.zeros(M, 64, device=dev)
     add = torch.randn(M, 256, device=dev)
-    V1.copy_(add)
-    chain(Mat(G), 256, [CL(L2, ops.EK_DACT_SOFTPLUS, 256, transposed=True, oscale=0.70710678, H=Mat(H2), hscale=1.41421356, ncol_main=217,
-                           tail=Mat(TL), save=Mat(V2)),
-                        CL(L1, ops.EK_DACT_SOFTPLUS, 256, transposed=True, H=Mat(H1), addend=Mat(V1), save=Mat(V1)),
-                        CL(L0, ops.EK_DACT_NONE, 39, transposed=True, save=Mat(U0))])
-    torch.cuda.synchronize()
     acc2 = G.double() @ W2
     s2 = dact_ref(H2.double()[:, :217] * 1.41421356, 1)
     g2 = 0.70710678 * s2 * acc2[:, :217]
     tl = 0.70710678 * acc2[:, 217:]
     g1 = dact_ref(H1.double(), 1) * (g2 @ W1) + add.double()
     g0 = g1 @ W0
-    for nm, got, want in [('g2', V2[:, :217], g2), ('tail', TL[:, :39], tl), ('g1', V1, g1), ('g0', U0[:, :39], g0)]:
-        e = float((got.double() - want).abs().max())
-        print(f'chain dact {nm}: max abs err {e:.2e} (|want| max {float(want.abs().max()):.2e})')
-        assert e < 3e-5 * max(1.0, float(want.abs().max()))
+    for fused in (True, False):
+        for t in (V2, U0, TL):
+            t.zero_()
+        V1.copy_(add)
+        mlp(Mat(G), [CL(L2, ops.EK_DACT_SOFTPLUS, 256, transposed=True, oscale=0.70710678, H=Mat(H2), hscale=1.41421356, ncol_main=217,
+                        tail=Mat(TL), save=Mat(V2)),
+                     CL(L1, ops.EK_DACT_SOFTPLUS, 256, transposed=True, H=Mat(H1), addend=Mat(V1), save=Mat(V1)),
+                     CL(L0, ops.EK_DACT_NONE, 39, transposed=True, save=Mat(U0))], fused=fused)
+        torch.cuda.synchronize()
+        for nm, got, want in [('g2', V2[:, :217], g2), ('tail', TL[:, :39], tl), ('g1', V1, g1), ('g0', U0[:, :39], g0)]:
+            e = float((got.double() - want).abs().max())
+            print(f'{"chain" if fused else "layerwise"} dact {nm}: max abs err {e:.2e} (|want| max {float(want.abs().max()):.2e})')
+            assert e < 3e-5 * max(1.0, float(want.abs().max()))
 
 
 @pytest.mark.parametrize('M', [1500, 40007])

@@ -189,6 +189,32 @@ def test_predict_materials_and_sdf_field_match_reference():
             net.extract_geometry(resolution=16)
 
 
+@pytest.fixture
+def per_layer(monkeypatch):
+    """The engine's per-layer MLP path: every pass expanded into one nero_linear launch per layer (USE_CHAIN = False)."""
+    from nero_b200 import engine
+    monkeypatch.setattr(engine, 'USE_CHAIN', False)
+
+
+@pytest.mark.parametrize('name', list(FIXTURE_CFGS))
+def test_render_core_per_layer_matches_reference(name, per_layer):
+    test_render_core_matches_reference(name)
+
+
+def test_sdf_values_per_layer_match_reference_1e4(per_layer):
+    test_sdf_values_match_reference_1e4()
+
+
+@pytest.mark.parametrize('name', list(VAL_FIXTURES))
+def test_validation_render_per_layer_matches_reference(name, per_layer):
+    test_validation_render_matches_reference(name)
+
+
+def test_predict_materials_per_layer_match_reference(per_layer):
+    """Fails when the per-layer path skips the SDF feature head that feeds the material predictors."""
+    test_predict_materials_and_sdf_field_match_reference()
+
+
 def test_standalone_encodings_match_reference():
     """nero_pe / nero_ide (the stand-alone entry points of the encodings) against the reference KATs, including directions
     within 1e-4 .. 5e-2 of the poles where the reference's fp32 l=16 band is 2.4e-3 away from exact arithmetic."""

@@ -92,7 +92,6 @@ def bench_chain_cases(dev, M, NL=8):
 def bell_step(dev):
     import bench
     from nero_b200 import synthetic as O
-    import nero_b200.engine as E
     net, _ = bench.build_net({}, dev)
     r = {k: v.to(dev).contiguous() for k, v in O.synthetic_rays(1024, seed=6033).items()}
     car = net.get_anneal_val(bench.STEP)
@@ -113,11 +112,11 @@ def bell_step(dev):
         orig(A0, k_valid0, layers, m_ptr, m_cap, tag=tag)
         ops.CHAIN_PHASES = None
         launches.append((tag or '-', FAMILY[layers[0]['kind']], buf, m_ptr, A0.t.shape[0] if m_cap is None else m_cap, len(layers)))
-    E.chain = chain
+    ops.chain = chain          # the engine's passes launch their chains through ops.mlp
     try:
         step()
     finally:
-        E.chain = orig
+        ops.chain = orig
     by = {}
     for tag, fam, buf, m_ptr, m_cap, nl in launches:
         rows = min(int(m_ptr.item()), m_cap) if m_ptr is not None else m_cap
