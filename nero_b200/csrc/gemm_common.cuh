@@ -85,7 +85,7 @@ __device__ __forceinline__ float2 ld2(const float* __restrict__ g, int ld, long 
   return x;
 }
 // an epilogue operand pointer may be null or must allow 8-byte pair loads
-inline bool pair_aligned(const float* g, int ld) {
+__host__ __device__ inline bool pair_aligned(const float* g, int ld) {
   return !g || ((reinterpret_cast<uintptr_t>(g) & 7) == 0 && (ld & 1) == 0);
 }
 // Written as three independently guarded stores rather than early returns, so that the compiler predicates them and the
@@ -129,17 +129,17 @@ __device__ __forceinline__ EpiIn epi_load(const EpiArgs& e, long row, int col, b
   return in;
 }
 
-// Epilogue of accumulator columns (col, col + 1) (col even) of one row, with its operands `in` from epi_load: writes
-// out / out2 / tail as the kind defines and returns the result values (those a following layer of a chain reads in the
-// main columns).  Rows that are not ok are computed with zero operands and not stored.
+// The arithmetic of accumulator columns (v0, v1) of one row with the bias (b0, b1) of those columns (bias kinds) or the
+// operands `in` (the others): returns the values `out` stores, but for the addend (epi_add), and in the tangent sweep
+// sets t to those out2 stores.  Both epilogue paths below run these same operations in this order, so they compute
+// bit-identical values.
 template <int KIND>
-__device__ __forceinline__ float2 epi_pair(const EpiArgs& e, long row, int col, bool row_ok, float v0, float v1, const EpiIn& in) {
+__device__ __forceinline__ float2 epi_values(const EpiArgs& e, float v0, float v1, float b0, float b1, const EpiIn& in, float2& t) {
   constexpr bool kBias = (KIND == EK_BIAS_SOFTPLUS || KIND == EK_BIAS_RELU || KIND == EK_BIAS_GENERIC);
-  const int nmain = kBias ? e.ncol_out : min(e.ncol_out, e.ncol_main);
   float r0, r1;
   if constexpr (kBias) {
-    float y0 = v0 + ((e.bias && col < e.n_bias) ? __ldg(e.bias + col) : 0.0f);
-    float y1 = v1 + ((e.bias && col + 1 < e.n_bias) ? __ldg(e.bias + col + 1) : 0.0f);
+    float y0 = v0 + b0;
+    float y1 = v1 + b1;
     if constexpr (KIND == EK_BIAS_SOFTPLUS) { y0 = softplus100_fast(y0); y1 = softplus100_fast(y1); }
     else if constexpr (KIND == EK_BIAS_RELU) { y0 = fmaxf(y0, 0.0f); y1 = fmaxf(y1, 0.0f); }
     else { y0 = apply_act(y0, e.act, e.act_param); y1 = apply_act(y1, e.act, e.act_param); }
@@ -156,21 +156,49 @@ __device__ __forceinline__ float2 epi_pair(const EpiArgs& e, long row, int col, 
     r1 = e.oscale * s1 * v1;
     if constexpr (KIND == EK_TANGENT) {
       const float2 v = in.v;
-      st2(e.out2, e.ldo2, row, col, nmain, row_ok, 100.0f * (1.0f - s0) * v.x * v0, 100.0f * (1.0f - s1) * v.y * v1);
+      t = make_float2(100.0f * (1.0f - s0) * v.x * v0, 100.0f * (1.0f - s1) * v.y * v1);
     }
+  }
+  return make_float2(r0, r1);
+}
+// the derivative-product epilogues' addend, added last
+template <int KIND>
+__device__ __forceinline__ void epi_add(const EpiArgs& e, const EpiIn& in, float2& r) {
+  constexpr bool kBias = (KIND == EK_BIAS_SOFTPLUS || KIND == EK_BIAS_RELU || KIND == EK_BIAS_GENERIC);
+  if constexpr (!kBias) {
     if (e.addend) {
       const float2 a = in.a;
-      r0 += a.x;
-      r1 += a.y;
+      r.x += a.x;
+      r.y += a.y;
     }
+  }
+}
+
+// Epilogue of accumulator columns (col, col + 1) of one row, with its operands `in` from epi_load: writes
+// out / out2 / tail as the kind defines and returns the result values (those a following layer of a chain reads in the
+// main columns).  Rows that are not ok are computed with zero operands and not stored.
+template <int KIND>
+__device__ __forceinline__ float2 epi_pair(const EpiArgs& e, long row, int col, bool row_ok, float v0, float v1, const EpiIn& in) {
+  constexpr bool kBias = (KIND == EK_BIAS_SOFTPLUS || KIND == EK_BIAS_RELU || KIND == EK_BIAS_GENERIC);
+  const int nmain = kBias ? e.ncol_out : min(e.ncol_out, e.ncol_main);
+  float b0 = 0.0f, b1 = 0.0f;
+  if constexpr (kBias) {
+    b0 = (e.bias && col < e.n_bias) ? __ldg(e.bias + col) : 0.0f;
+    b1 = (e.bias && col + 1 < e.n_bias) ? __ldg(e.bias + col + 1) : 0.0f;
+  }
+  float2 t;
+  float2 r = epi_values<KIND>(e, v0, v1, b0, b1, in, t);
+  if constexpr (KIND == EK_TANGENT) st2(e.out2, e.ldo2, row, col, nmain, row_ok, t.x, t.y);
+  epi_add<KIND>(e, in, r);
+  if constexpr (!kBias) {
     // skip-branch columns [ncol_main, ncol_out) carry oscale * acc and go to the tail buffer
     if (e.tail && row_ok) {
       if (col >= e.ncol_main && col < e.ncol_out) __stcs(e.tail + row * e.ldt + (col - e.ncol_main), e.oscale * v0);
       if (col + 1 >= e.ncol_main && col + 1 < e.ncol_out) __stcs(e.tail + row * e.ldt + (col + 1 - e.ncol_main), e.oscale * v1);
     }
   }
-  st2(e.out, e.ldo, row, col, nmain, row_ok, r0, r1);
-  return make_float2(col < nmain ? r0 : 0.0f, col + 1 < nmain ? r1 : 0.0f);
+  st2(e.out, e.ldo, row, col, nmain, row_ok, r.x, r.y);
+  return make_float2(col < nmain ? r.x : 0.0f, col + 1 < nmain ? r.y : 0.0f);
 }
 
 // Column blocks (8 accumulator columns each) whose operand loads a thread issues back to back.  An epilogue that loads
@@ -211,6 +239,48 @@ __device__ __forceinline__ void epi_fragment(const EpiArgs& e, long row0, bool o
 #pragma unroll
       for (int h = 0; h < 2; ++h)
         body(g * G + j, h, row0 + 8 * h, 8 * (g * G + j) + 2 * (lane & 3), h ? ok1 : ok0, in[g & 1][2 * j + h]);
+  }
+}
+
+// ---- plain layers.  A chain layer is plain when none of the per-pair tests of epi_load / epi_pair / st2 can fail for it
+// (k_gemm_chain.cu: chain_layer); then each operand row is one pointer per thread, every column a compile-time offset from
+// it, and only the row tests remain.  `ok`: the row exists; `add`: it exists and the layer has an addend.
+struct PlainRows {
+  const float* h[2]; const float* v[2]; const float* a[2];
+  bool ok[2], add[2];
+};
+// the operands of columns (c, c + 1) of this thread's row row0 + 8 h, c relative to the row pointers of `pr`
+template <int KIND>
+__device__ __forceinline__ EpiIn plain_load(const PlainRows& pr, int h, int c) {
+  constexpr bool kBias = (KIND == EK_BIAS_SOFTPLUS || KIND == EK_BIAS_RELU || KIND == EK_BIAS_GENERIC);
+  EpiIn in{make_float2(0.f, 0.f), make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
+  if constexpr (!kBias) {
+    if constexpr (KIND != EK_DACT_NONE) if (pr.ok[h]) in.h = __ldcs(reinterpret_cast<const float2*>(pr.h[h] + c));
+    if constexpr (KIND == EK_TANGENT) if (pr.ok[h]) in.v = __ldcs(reinterpret_cast<const float2*>(pr.v[h] + c));
+    if constexpr (KIND != EK_TANGENT) if (pr.add[h]) in.a = __ldcs(reinterpret_cast<const float2*>(pr.a[h] + c));
+  }
+  return in;
+}
+// epi_fragment for a plain layer: body(jb, h, in) for all NB column blocks, with the same group-ahead loads
+template <int KIND, int NB, class Body>
+__device__ __forceinline__ void epi_fragment_plain(const PlainRows& pr, Body&& body) {
+  constexpr int G = NB < kEpiGroup<KIND> ? NB : kEpiGroup<KIND>;
+  static_assert(NB % G == 0, "whole groups of column blocks");
+  EpiIn in[2][2 * G];
+  auto load = [&](int g, EpiIn* dst) {
+#pragma unroll
+    for (int j = 0; j < G; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) dst[2 * j + h] = plain_load<KIND>(pr, h, 8 * (g * G + j));
+  };
+  load(0, in[0]);
+#pragma unroll
+  for (int g = 0; g < NB / G; ++g) {
+    if (g + 1 < NB / G) load(g + 1, in[(g + 1) & 1]);
+#pragma unroll
+    for (int j = 0; j < G; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) body(g * G + j, h, in[g & 1][2 * j + h]);
   }
 }
 

@@ -169,30 +169,82 @@ __device__ __forceinline__ void chain_layer(const nero_chain_params& p, const ne
 
   const EpiArgs e{L.bias, L.n_bias, L.save, L.ld_save, L.H, L.ldh, L.hscale, KIND == EK_TANGENT ? nullptr : L.addend, L.ldadd,
                   L.V, L.ldv, L.out2, L.ldo2, L.tail, L.ldt, L.ncol_out, L.ncol_main, L.oscale, L.act, L.act_param};
-  const int nmain = kBias ? L.ncol_out : min(L.ncol_out, L.ncol_main);
-  const int n_a = L.write_a ? max(L.a_blocks * 16, L.n_pad) : 0;       // next-A columns to define
-  const float* csrc = L.csrc;
-  const int ld_csrc = L.ld_csrc;
-  const bool skip_cols = csrc && nmain < n_a;                            // some of them come from csrc
   const int rl0 = c.wg * 64 + c.w * 16 + (c.l >> 2);
-  epi_fragment<KIND, 2 * HN / 8>(e, long(tile) * CH_BM + rl0, rl0 < rows_valid, rl0 + 8 < rows_valid, c.l, nh * (HN / 8),
-                                 [&](int jb, int h, long row, int col, bool row_ok, const EpiIn& in) {
-    const int hf = jb / (HN / 8), i = 4 * (jb % (HN / 8)) + 2 * h;
-    // zeros at and beyond ncol_out (>= the main columns), where it stores nothing: no branch around it
-    float2 r = epi_pair<KIND>(e, row, col, row_ok, acc[hf][i], acc[hf][i + 1], in);
-    // next-A columns >= nmain come from csrc (r is zero there); loads and stores are predicated, not branched around
-    const float* q = csrc + row * ld_csrc + col;
-    if (skip_cols && row_ok && col >= nmain) r.x = __ldcs(q);
-    if (skip_cols && row_ok && col + 1 >= nmain) r.y = __ldcs(q + 1);
-    put_a2(c.s_a, rl0 + 8 * h, col, r.x, r.y, col < n_a);
-  });
-  // next-A columns beyond the accumulator (skip-concat source or zero): each warp fills its own 16 rows
-  const int extra = (n_a - L.n_pad) >> 1;
-  for (int i = c.l; i < 16 * extra; i += 32) {
-    const int rl = c.wg * 64 + c.w * 16 + i / extra, col = L.n_pad + 2 * (i % extra);
-    const long row = long(tile) * CH_BM + rl;
-    const bool row_ok = rl < rows_valid;
-    put_a2(c.s_a, rl, col, csrc_at(L, row, col, row_ok), csrc_at(L, row, col + 1, row_ok));
+  const bool ok0 = rl0 < rows_valid, ok1 = rl0 + 8 < rows_valid;
+  // Plain layer: all 256 accumulator columns are main columns (no tail, no skip-concat columns, next A exactly 256 wide),
+  // every bias column exists, and the outputs take 8-byte pair stores (H, V and the addend do: checked at launch).  Then
+  // no column test of the general epilogue below can fail, and the plain one runs without them.  The SDF, NeRF and
+  // predictor hidden layers of every pass are plain; the skip layer, the heads and the 39-wide first layers are not.
+  const bool plain = L.n_pad == 2 * HN && L.ncol_out == 2 * HN && (kBias || L.ncol_main >= 2 * HN) &&
+                     (!kBias || !L.bias || L.n_bias >= 2 * HN) && pair_aligned(L.save, L.ld_save) &&
+                     (KIND != EK_TANGENT || pair_aligned(L.out2, L.ldo2));
+  if (plain) {
+    // row pointers at this thread's column 2 (l % 4) of its rows; the columns of its pairs are immediates off them
+    const int c0 = 2 * (c.l & 3);
+    PlainRows pr;
+    float* out[2];
+    float* out2[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const long row = long(tile) * CH_BM + rl0 + 8 * h;
+      pr.h[h] = L.H + row * L.ldh + c0;
+      pr.v[h] = L.V + row * L.ldv + c0;
+      pr.a[h] = e.addend + row * L.ldadd + c0;
+      pr.ok[h] = h ? ok1 : ok0;
+      pr.add[h] = pr.ok[h] && e.addend;
+      out[h] = L.save + row * L.ld_save + c0;
+      out2[h] = L.out2 + row * L.ldo2 + c0;
+    }
+    const bool st_out = L.save != nullptr, st_a = L.write_a;
+    const float* bias = L.bias + c0;
+    // next-A byte address of column 8 jb + c0 of row rl0 + 8 h: sw128_offset's 16-byte unit (jb & 7) ^ (rl0 & 7) is
+    // a_row ^ ((jb & 7) << 4) (bits 4-6 of a_row hold rl0 & 7, and nothing else of it is in those bits); the 64-wide
+    // chunk jb / 8 and the row offset h are immediates
+    const uint32_t a_row = (smem_u32(c.s_a) + rl0 * 128 + 2 * c0) | ((rl0 & 7) << 4);
+    epi_fragment_plain<KIND, 2 * HN / 8>(pr, [&](int jb, int h, const EpiIn& in) {
+      const int hf = jb / (HN / 8), i = 4 * (jb % (HN / 8)) + 2 * h;
+      float b0 = 0.0f, b1 = 0.0f;
+      if constexpr (kBias) {    // two 4-byte loads: a bias is a view of a parameter buffer and need not be 8-byte aligned
+        if (L.bias) { b0 = __ldg(bias + 8 * jb); b1 = __ldg(bias + 8 * jb + 1); }
+      }
+      float2 t;
+      float2 r = epi_values<KIND>(e, acc[hf][i], acc[hf][i + 1], b0, b1, in, t);
+      if constexpr (KIND == EK_TANGENT) {
+        if (pr.ok[h]) __stcs(reinterpret_cast<float2*>(out2[h] + 8 * jb), t);
+      }
+      epi_add<KIND>(e, in, r);
+      if (st_out && pr.ok[h]) __stcs(reinterpret_cast<float2*>(out[h] + 8 * jb), r);
+      uint32_t hi, lo;
+      split2(r.x, r.y, hi, lo);
+      const uint32_t q = (a_row ^ ((jb & 7) << 4)) + (jb >> 3) * (2 * kAPlane) + h * (8 * 128);
+      sts_u32_if(q, hi, st_a);
+      sts_u32_if(q + kAPlane, lo, st_a);
+    });
+  } else {
+    const int nmain = kBias ? L.ncol_out : min(L.ncol_out, L.ncol_main);
+    const int n_a = L.write_a ? max(L.a_blocks * 16, L.n_pad) : 0;       // next-A columns to define
+    const float* csrc = L.csrc;
+    const int ld_csrc = L.ld_csrc;
+    const bool skip_cols = csrc && nmain < n_a;                            // some of them come from csrc
+    epi_fragment<KIND, 2 * HN / 8>(e, long(tile) * CH_BM + rl0, ok0, ok1, c.l, nh * (HN / 8),
+                                   [&](int jb, int h, long row, int col, bool row_ok, const EpiIn& in) {
+      const int hf = jb / (HN / 8), i = 4 * (jb % (HN / 8)) + 2 * h;
+      // zeros at and beyond ncol_out (>= the main columns), where it stores nothing: no branch around it
+      float2 r = epi_pair<KIND>(e, row, col, row_ok, acc[hf][i], acc[hf][i + 1], in);
+      // next-A columns >= nmain come from csrc (r is zero there); loads and stores are predicated, not branched around
+      const float* q = csrc + row * ld_csrc + col;
+      if (skip_cols && row_ok && col >= nmain) r.x = __ldcs(q);
+      if (skip_cols && row_ok && col + 1 >= nmain) r.y = __ldcs(q + 1);
+      put_a2(c.s_a, rl0 + 8 * h, col, r.x, r.y, col < n_a);
+    });
+    // next-A columns beyond the accumulator (skip-concat source or zero): each warp fills its own 16 rows
+    const int extra = (n_a - L.n_pad) >> 1;
+    for (int i = c.l; i < 16 * extra; i += 32) {
+      const int rl = c.wg * 64 + c.w * 16 + i / extra, col = L.n_pad + 2 * (i % extra);
+      const long row = long(tile) * CH_BM + rl;
+      const bool row_ok = rl < rows_valid;
+      put_a2(c.s_a, rl, col, csrc_at(L, row, col, row_ok), csrc_at(L, row, col + 1, row_ok));
+    }
   }
   fence_proxy_async_smem();
   CH_PHASE(li, PH_EPI, t_ph);
