@@ -4,7 +4,8 @@ stages.
 Reference being replaced (paths relative to the reference repository):
   run_colmap.py:66-90   image_undistorter, patch_match_stereo and stereo_fusion, which write <project>/points.ply, the cloud
                         custom_object.md crops by hand (and tools/prepare_custom_object.py crops here)
-patch_match_stereo exists only in CUDA builds of COLMAP.  This module restates COLMAP's PatchMatch in spirit (a plane per
+patch_match_stereo exists only in CUDA builds of COLMAP.  The workflow is tools/match_features.py (nero_b200.features)
+-> colmap mapper -> tools/dense_points.py -> tools/prepare_custom_object.py.  This module restates COLMAP's PatchMatch in spirit (a plane per
 pixel, NCC over plane-induced homographies, red-black propagation, forward-backward geometric filtering); it is not pinned
 to COLMAP's output (DESIGN.md section 2).
 
@@ -182,9 +183,10 @@ def select_sources(points, tracks, poses, image_ids, sources=SOURCES, angles=(AN
 
 
 def read_rgb(path):
-    """uint8 RGB [h,w,3] of an image file."""
+    """uint8 RGB [h,w,3] of an image file, in its stored pixel order: an EXIF orientation is ignored, as COLMAP and
+    run_colmap.py's skimage reader ignore it, so the pixels are in the frame of the COLMAP model's cameras."""
     import cv2
-    img = cv2.imread(path, cv2.IMREAD_COLOR)
+    img = cv2.imread(path, cv2.IMREAD_COLOR | cv2.IMREAD_IGNORE_ORIENTATION)
     if img is None:
         raise FileNotFoundError(f'{path}: cannot read the image')
     return np.ascontiguousarray(img[..., ::-1])
