@@ -1,6 +1,6 @@
 """Sparse features on the GPU: SIFT extraction, all-pair matching and two-view verification of a custom object's images,
-written as the COLMAP database that `colmap mapper` reconstructs from, without COLMAP's feature_extractor or
-exhaustive_matcher.
+written as the COLMAP database that nero_b200.sfm (tools/map_sparse.py) or `colmap mapper` reconstructs from, without
+COLMAP's feature_extractor or exhaustive_matcher.
 
 Reference being replaced (paths relative to the reference repository):
   run_colmap.py:12-39   database.db with one SIMPLE_PINHOLE camera per image (or one shared camera with --same_camera)

@@ -5,7 +5,7 @@ Reference being replaced (paths relative to the reference repository):
   run_colmap.py:66-90   image_undistorter, patch_match_stereo and stereo_fusion, which write <project>/points.ply, the cloud
                         custom_object.md crops by hand (and tools/prepare_custom_object.py crops here)
 patch_match_stereo exists only in CUDA builds of COLMAP.  The workflow is tools/match_features.py (nero_b200.features)
--> colmap mapper -> tools/dense_points.py -> tools/prepare_custom_object.py.  This module restates COLMAP's PatchMatch in spirit (a plane per
+-> tools/map_sparse.py (nero_b200.sfm; or colmap mapper) -> tools/dense_points.py -> tools/prepare_custom_object.py.  This module restates COLMAP's PatchMatch in spirit (a plane per
 pixel, NCC over plane-induced homographies, red-black propagation, forward-backward geometric filtering); it is not pinned
 to COLMAP's output (DESIGN.md section 2).
 

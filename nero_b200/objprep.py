@@ -176,6 +176,35 @@ def read_colmap_model(path, tracks=False):
     return views, np.asarray(pts, np.float64).reshape(-1, 3)
 
 
+def write_colmap_model(path, cameras, images, points):
+    """Write cameras.bin, images.bin and points3D.bin in `path` (created if missing), in the dicts' order.
+    cameras: {id: (model name, width, height, params)}; images: {id: (qvec (w, x, y, z), tvec, camera_id, name, xys [k, 2],
+    point3D_ids [k] (-1: none))}; points: {id: (xyz, rgb, error, image_ids, point2D_idxs)}."""
+    ids = {name: (mid, npar) for mid, (name, npar) in CAMERA_MODELS.items()}
+    os.makedirs(path, exist_ok=True)
+    with open(os.path.join(path, 'cameras.bin'), 'wb') as f:
+        f.write(struct.pack('<Q', len(cameras)))
+        for cid, (model, w, h, params) in cameras.items():
+            mid, npar = ids[model]
+            if len(params) != npar:
+                raise ValueError(f'camera {cid}: {model} takes {npar} parameters, not {len(params)}')
+            f.write(struct.pack('<iiQQ', cid, mid, w, h) + struct.pack(f'<{npar}d', *params))
+    with open(os.path.join(path, 'images.bin'), 'wb') as f:
+        f.write(struct.pack('<Q', len(images)))
+        for iid, (q, t, cid, name, xys, p3d) in images.items():
+            xys = np.asarray(xys, np.float64).reshape(-1, 2)
+            p3d = np.asarray(p3d, np.int64).reshape(-1)
+            f.write(struct.pack('<i4d3di', iid, *q, *t, cid) + name.encode('utf-8') + b'\x00' + struct.pack('<Q', p3d.shape[0]))
+            rec = np.zeros(p3d.shape[0], np.dtype([('x', '<f8'), ('y', '<f8'), ('id', '<i8')]))
+            rec['x'], rec['y'], rec['id'] = xys[:, 0], xys[:, 1], p3d
+            f.write(rec.tobytes())
+    with open(os.path.join(path, 'points3D.bin'), 'wb') as f:
+        f.write(struct.pack('<Q', len(points)))
+        for pid, (xyz, rgb, err, iids, p2d) in points.items():
+            f.write(struct.pack('<Q3d3Bd', pid, *xyz, *rgb, err) + struct.pack('<Q', len(iids)))
+            f.write(np.stack([np.asarray(iids, '<i4'), np.asarray(p2d, '<i4')], 1).tobytes())
+
+
 # ------------------------------------------------------------------------------------------------ cameras and scale
 def camera_centers(views):
     """(names [n] in name order, centres fp64 [n,3], optical axes fp64 [n,3]) of the views, from their float32 poses."""

@@ -6,8 +6,8 @@
 Replaces the dense half of run_colmap.py (image_undistorter, patch_match_stereo, stereo_fusion), which needs a CUDA build
 of COLMAP: PatchMatch stereo per view, a forward-backward geometric filter against the source views, and the surviving
 pixels unprojected into one cloud.  The output goes where run_colmap.py writes its fused cloud, so
-tools/prepare_custom_object.py finds it there.  The workflow becomes: match_features.py -> colmap mapper ->
-dense_points.py -> prepare_custom_object.py.  The protocol and its defaults are stated in nero_b200/mvs.py.
+tools/prepare_custom_object.py finds it there.  The workflow becomes: match_features.py -> map_sparse.py (or colmap
+mapper) -> dense_points.py -> prepare_custom_object.py.  The protocol and its defaults are stated in nero_b200/mvs.py.
 
 --sparse defaults to <root>/colmap/sparse/0, else <root>/sparse/0; --images to <root>/images.  --voxel (COLMAP units)
 thins the cloud to one point per voxel.  Views without enough source views or sparse points are skipped and reported.

@@ -1,4 +1,4 @@
-"""Extract and match SIFT features of a custom object's images on the GPU: <root>/database.db, ready for `colmap mapper`.
+"""Extract and match SIFT features of a custom object's images on the GPU: <root>/database.db, ready for map_sparse.py.
 
     python tools/match_features.py --root data/custom/kettle [--images <dir>] [--same_camera] [--max-size 3200]
         [--max-features 8192] [--force]
@@ -6,8 +6,9 @@
 Replaces the first three steps of run_colmap.py: the database with one SIMPLE_PINHOLE camera per image (or one shared
 camera with --same_camera), COLMAP's feature_extractor and its exhaustive_matcher.  The database holds the cameras,
 images, keypoints, descriptors, the matches of every image pair and the verified two-view geometries, in COLMAP's
-schema.  The only COLMAP step left is `colmap mapper`, which runs on the CPU in every build of COLMAP; the tool prints
-that command.  The workflow becomes: match_features.py -> colmap mapper -> dense_points.py -> prepare_custom_object.py.
+schema.  The next step is map_sparse.py, the GPU mapper (COLMAP's CPU `colmap mapper` reads the same database); the
+tool prints both commands.  The workflow becomes: match_features.py -> map_sparse.py -> dense_points.py ->
+prepare_custom_object.py.
 The protocol and its defaults are stated in nero_b200/features.py.
 """
 import argparse
@@ -53,7 +54,9 @@ def main(argv=None):
           f'{info["verified"]} verified (extract {t["extract"]:.2f} s, match {t["match"]:.2f} s, verify {t["verify"]:.2f} s, '
           f'write {t["write"]:.2f} s)')
     os.makedirs(os.path.join(flags.root, 'sparse'), exist_ok=True)
-    print('next: colmap mapper --database_path {0}/database.db --image_path {1} --output_path {0}/sparse'.format(flags.root, flags.images))
+    print(f'next: python tools/map_sparse.py --root {flags.root}')
+    print('  (or COLMAP\'s CPU mapper: colmap mapper --database_path {0}/database.db --image_path {1} --output_path {0}/sparse)'
+          .format(flags.root, flags.images))
     return info
 
 
