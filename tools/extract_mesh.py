@@ -1,6 +1,7 @@
 """Stage-I checkpoint -> triangle mesh for stage II, on the GPU (the reference's extract_mesh.py).
 
     python tools/extract_mesh.py --cfg configs/shape/syn/bell.yaml [--resolution 512] [--sparse [--brick 8] [--lipschitz 2.0]]
+                                 [--faces N]
 
 Loads data/model/<name>/model.pth ({'step', 'network_state_dict', ...}), samples the SDF on a resolution^3 grid over [-1,1]^3
 (1.0 outside the unit sphere), runs marching cubes at level 0 and writes data/meshes/<name>-<step>.ply, the path
@@ -10,6 +11,10 @@ With --sparse the SDF is sampled only in bricks of brick^3 cubes around the surf
 the same mesh, at a cost that follows the surface, which is what makes --resolution 1024 and 2048 possible on one card.  A
 closed piece of surface smaller than a brick where the SDF is steeper than --lipschitz can be missed; raise --lipschitz or
 lower --brick then.
+
+With --faces N the mesh is reduced to about N triangles by quadric edge collapse (nero_b200/simplify.py) before it is
+written, to the same path: `--sparse --resolution 2048 --faces 888056` gives a stage-II-sized mesh that keeps the detail
+of the fine grid where the surface curves.
 """
 import argparse
 import os
@@ -27,7 +32,10 @@ def main(argv=None):
     parser.add_argument('--sparse', action='store_true', help='sample the SDF in a narrow band around the surface only')
     parser.add_argument('--brick', type=int, default=8, choices=(4, 8, 16), help='cubes per brick edge (with --sparse)')
     parser.add_argument('--lipschitz', type=float, default=2.0, help='bound on the SDF slope used for seeding (with --sparse)')
+    parser.add_argument('--faces', type=int, default=None, help='simplify the mesh to about this many triangles (>= 4)')
     flags = parser.parse_args(argv)
+    if flags.faces is not None and flags.faces < 4:
+        raise SystemExit(f'extract_mesh: --faces must be >= 4, got {flags.faces}')
 
     import torch
     import yaml
@@ -51,12 +59,20 @@ def main(argv=None):
                                                                  lipschitz=flags.lipschitz, return_stats=True)
     else:
         vertices, triangles = network.extract_mesh(resolution=flags.resolution, threshold=0.0)
+    simplified = None
+    if flags.faces is not None:
+        from nero_b200.simplify import simplify, stats_line
+        n_in = triangles.shape[0]
+        vertices, triangles, simplified = simplify(vertices, triangles, flags.faces)
+        print(f'simplified {n_in} -> {triangles.shape[0]} triangles')
     os.makedirs('data/meshes', exist_ok=True)
     path = os.path.join('data', 'meshes', f'{cfg["name"]}-{step}.ply')
     write_ply(path, vertices, triangles)
     print(f'{path}: {vertices.shape[0]} vertices, {triangles.shape[0]} triangles')
     if stats is not None:
         print('sparse: ' + ', '.join(f'{k} {v}' for k, v in stats.items()))
+    if simplified is not None:
+        print(stats_line(simplified))
     return path
 
 
