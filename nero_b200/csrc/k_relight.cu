@@ -8,9 +8,12 @@
 // Per path: jittered camera ray -> closest hit; at each hit, next-event estimation from the importance-sampled environment
 // with an any-hit shadow ray, and a BRDF sample (diffuse or GGX lobe) that continues the path; the two are combined with
 // the power heuristic.  No Russian roulette: at most 1 + 2 * max_bounces rays per path.
+// The kAov instances also add each hitting sample's first-hit guides and demodulated radiance into the feature sums the
+// denoiser reads (include/nero_denoise.h); they only read values the colour path computes, so accum keeps its bits.
 #include "bvh_traverse.cuh"
 #include "common.cuh"
 #include "math_relight.cuh"
+#include "../../include/nero_denoise.h"
 #include "../../include/nero_relight_tex.h"
 
 namespace nero {
@@ -102,8 +105,8 @@ __device__ __forceinline__ float mis(float a, float b) {   // power heuristic a^
   return a2 / (a2 + b * b);
 }
 
-template <class Materials>
-__global__ void __launch_bounds__(128) relight_kernel(const nero_relight_params q, const Materials mat) {
+template <class Materials, bool kAov>
+__global__ void __launch_bounds__(128) relight_kernel(const nero_relight_params q, const Materials mat, float4* aov) {
   const int x = blockIdx.x * 16 + (threadIdx.x & 15), y = blockIdx.y * 8 + (threadIdx.x >> 4);
   if (x >= q.width || y >= q.height) return;
   const uint32_t pix = uint32_t(y) * uint32_t(q.width) + uint32_t(x);
@@ -113,6 +116,10 @@ __global__ void __launch_bounds__(128) relight_kernel(const nero_relight_params 
   const int W = q.env_w, H = q.env_h;
   const float* R = q.pose;
   float4 acc = reinterpret_cast<float4*>(q.accum)[pix];
+  float4 f_dem, f_alb, f_nrm, f_pos;   // feature sums (kAov only)
+  if (kAov) {
+    f_dem = aov[4 * pix]; f_alb = aov[4 * pix + 1]; f_nrm = aov[4 * pix + 2]; f_pos = aov[4 * pix + 3];
+  }
   unsigned long long rays = 0;
   for (int s = q.spp0; s < q.spp0 + q.spp; ++s) {
     const uint32_t si = uint32_t(s);
@@ -129,6 +136,24 @@ __global__ void __launch_bounds__(128) relight_kernel(const nero_relight_params 
     BvhHit h = bvh_traverse<false>(n4, tris, o[0], o[1], o[2], d[0], d[1], d[2], 1e30f);
     if (h.tri < 0) continue;                      // transparent film: background seen directly contributes nothing
     float L[3] = {0.f, 0.f, 0.f}, thr[3] = {1.f, 1.f, 1.f};
+    float g[3], n0[3], p0[3], z0;        // first-hit guides (kAov only)
+    if (kAov) {
+      // Taken from a surface() of their own before the bounce loop, of a copy of the hit the compiler cannot see through,
+      // and written with _rn intrinsics, which are never fused: a branch or a select on the bounce index inside the loop, or
+      // a surface() the compiler can merge with the loop's first one, changes how it splits and fuses the colour path's
+      // multiplies and adds, and so accum's bits.
+      BvhHit h0 = h;
+      asm("" : "+r"(h0.tri), "+f"(h0.t), "+f"(h0.u), "+f"(h0.v));
+      SurfHit s0;
+      surface(q, mat, h0, o, d, s0);
+      const float m = s0.metallic, m1 = __fsub_rn(1.0f, m), f0 = __fmul_rn(0.04f, m1);
+      for (int k = 0; k < 3; ++k) {
+        g[k] = __fadd_rn(__fadd_rn(__fmul_rn(m1, s0.albedo[k]), f0), __fmul_rn(m, s0.albedo[k]));
+        n0[k] = s0.n[k];
+        p0[k] = s0.p[k];
+      }
+      z0 = __fmul_rn(h0.t, __fadd_rn(__fadd_rn(__fmul_rn(R[8], d[0]), __fmul_rn(R[9], d[1])), __fmul_rn(R[10], d[2])));
+    }
     for (int b = 0; b < q.max_bounces; ++b) {
       SurfHit sh;
       surface(q, mat, h, o, d, sh);
@@ -195,8 +220,22 @@ __global__ void __launch_bounds__(128) relight_kernel(const nero_relight_params 
     acc.y = __fadd_rn(acc.y, L[1]);
     acc.z = __fadd_rn(acc.z, L[2]);
     acc.w = __fadd_rn(acc.w, 1.0f);
+    if (kAov) {
+      float D[3];
+      for (int k = 0; k < 3; ++k) D[k] = __fdiv_rn(L[k], __fadd_rn(g[k], NERO_DENOISE_DEMOD_EPS));
+      const float l = __fadd_rn(__fadd_rn(__fmul_rn(0.2126f, D[0]), __fmul_rn(0.7152f, D[1])), __fmul_rn(0.0722f, D[2]));
+      f_dem.x = __fadd_rn(f_dem.x, D[0]); f_dem.y = __fadd_rn(f_dem.y, D[1]); f_dem.z = __fadd_rn(f_dem.z, D[2]);
+      f_dem.w = __fadd_rn(f_dem.w, __fmul_rn(l, l));
+      f_alb.x = __fadd_rn(f_alb.x, g[0]); f_alb.y = __fadd_rn(f_alb.y, g[1]); f_alb.z = __fadd_rn(f_alb.z, g[2]);
+      f_nrm.x = __fadd_rn(f_nrm.x, n0[0]); f_nrm.y = __fadd_rn(f_nrm.y, n0[1]); f_nrm.z = __fadd_rn(f_nrm.z, n0[2]);
+      f_pos.x = __fadd_rn(f_pos.x, p0[0]); f_pos.y = __fadd_rn(f_pos.y, p0[1]); f_pos.z = __fadd_rn(f_pos.z, p0[2]);
+      f_pos.w = __fadd_rn(f_pos.w, z0);
+    }
   }
   reinterpret_cast<float4*>(q.accum)[pix] = acc;
+  if (kAov) {
+    aov[4 * pix] = f_dem; aov[4 * pix + 1] = f_alb; aov[4 * pix + 2] = f_nrm; aov[4 * pix + 3] = f_pos;
+  }
   if (q.rays) atomicAdd(q.rays, rays);
 }
 
@@ -206,11 +245,11 @@ bool scene_ok(const nero_relight_params& q) {
   return q.env_w >= 1 && q.env_h >= 1 && q.width >= 1 && q.height >= 1 && q.spp0 >= 0 && q.spp >= 0 && q.max_bounces >= 1;
 }
 
-template <class Materials>
-int launch(const nero_relight_params& q, const Materials& m, void* stream) {
+template <bool kAov, class Materials>
+int launch(const nero_relight_params& q, const Materials& m, float* aov, void* stream) {
   if (q.spp == 0) return NERO_OK;
   const dim3 grid((q.width + 15) / 16, (q.height + 7) / 8);
-  relight_kernel<<<grid, 128, 0, (cudaStream_t)stream>>>(q, m);
+  relight_kernel<Materials, kAov><<<grid, 128, 0, (cudaStream_t)stream>>>(q, m, reinterpret_cast<float4*>(aov));
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
@@ -219,14 +258,26 @@ int launch(const nero_relight_params& q, const Materials& m, void* stream) {
 
 extern "C" int nero_relight_render(const nero_relight_params* p, void* stream) {
   if (!p || !p->vmat || !scene_ok(*p)) return NERO_ERR_ARG;
-  return launch(*p, VertexMaterials{}, stream);
+  return launch<false>(*p, VertexMaterials{}, nullptr, stream);
 }
 
 extern "C" int nero_relight_render_textured(const nero_relight_params* p, const float* vt, const int* ft, int n_uv, const float* tex,
                                             int tex_w, int tex_h, void* stream) {
   if (!p || p->vmat || !scene_ok(*p) || !vt || !ft || !tex || n_uv < 1 || tex_w < 1 || tex_h < 1) return NERO_ERR_ARG;
   const TexMaterials m{reinterpret_cast<const float2*>(vt), ft, reinterpret_cast<const float4*>(tex), tex_w, tex_h};
-  return launch(*p, m, stream);
+  return launch<false>(*p, m, nullptr, stream);
+}
+
+extern "C" int nero_relight_render_aov(const nero_relight_params* p, float* aov, void* stream) {
+  if (!p || !p->vmat || !scene_ok(*p) || !aov) return NERO_ERR_ARG;
+  return launch<true>(*p, VertexMaterials{}, aov, stream);
+}
+
+extern "C" int nero_relight_render_textured_aov(const nero_relight_params* p, const float* vt, const int* ft, int n_uv,
+                                                const float* tex, int tex_w, int tex_h, float* aov, void* stream) {
+  if (!p || p->vmat || !scene_ok(*p) || !vt || !ft || !tex || n_uv < 1 || tex_w < 1 || tex_h < 1 || !aov) return NERO_ERR_ARG;
+  const TexMaterials m{reinterpret_cast<const float2*>(vt), ft, reinterpret_cast<const float4*>(tex), tex_w, tex_h};
+  return launch<true>(*p, m, aov, stream);
 }
 
 }  // namespace nero

@@ -27,6 +27,7 @@ _MVS_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_mvs.h')  # s
 _FEATURES_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_features.h')  # same library, plain-argument entry points
 _SFM_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_sfm.h')  # same library, plain-argument entry points
 _SIMPLIFY_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_simplify.h')  # same library, plain-argument entry points
+_DENOISE_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_denoise.h')  # same library, plain-argument entry points
 
 ACT_NONE, ACT_SOFTPLUS100, ACT_RELU, ACT_SIGMOID, ACT_EXPCLAMP = 0, 1, 2, 3, 4
 EPI_BIAS_ACT, EPI_MUL_DACT, EPI_TANGENT = 0, 1, 2
@@ -122,10 +123,12 @@ MVS_PROTOS = _parse_header(_MVS_HEADER)[1]
 FEATURES_PROTOS = _parse_header(_FEATURES_HEADER)[1]
 SFM_PROTOS = _parse_header(_SFM_HEADER)[1]
 SIMPLIFY_PROTOS = _parse_header(_SIMPLIFY_HEADER)[1]
+DENOISE_PROTOS = _parse_header(_DENOISE_HEADER)[1]
 for _name, _argtypes in (list(_PROTOS.items()) + list(TEXMAP_PROTOS.items()) + list(ENVMAP_PROTOS.items()) +
                          list(METRICS_PROTOS.items()) + list(RELIGHT_TEX_PROTOS.items()) + list(MESHPTS_PROTOS.items()) +
                          list(OBJPREP_PROTOS.items()) + list(MCSPARSE_PROTOS.items()) + list(MVS_PROTOS.items()) +
-                         list(FEATURES_PROTOS.items()) + list(SFM_PROTOS.items()) + list(SIMPLIFY_PROTOS.items())):
+                         list(FEATURES_PROTOS.items()) + list(SFM_PROTOS.items()) + list(SIMPLIFY_PROTOS.items()) +
+                         list(DENOISE_PROTOS.items())):
     _fn = getattr(lib, _name)
     _fn.argtypes, _fn.restype = _argtypes, ctypes.c_int
 # nero_abi_sizeof(i) is the size of ABI_RECORDS[i]; a library built from another version of the header would read the

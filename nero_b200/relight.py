@@ -492,15 +492,8 @@ class Relighter:
         self.env_d = {k: up(v) for k, v in self.tables.items()}
         self.rays = torch.zeros(1, dtype=torch.int64, device=self.dev)
 
-    def render(self, pose, K, h, w, spp, max_bounces=4, seed=0, spp_per_launch=16):
-        """One image -> CUDA float32 [h,w,4]: linear RGB premultiplied by coverage, alpha = fraction of camera samples that hit
-        the mesh.  pose: world -> camera [3,4] (OpenCV axes), K: [3,3] pinhole intrinsics.  The samples are launched in
-        chunks of spp_per_launch; the result does not depend on the chunking.  self.rays accumulates the rays traced."""
-        import torch
+    def _params(self, pose, K, h, w, max_bounces, seed, accum):
         from . import ops
-        if spp < 1 or max_bounces < 1 or spp_per_launch < 1:
-            raise ValueError('spp, max_bounces and spp_per_launch must be positive')
-        accum = torch.zeros(h * w, 4, device=self.dev)
         e = self.env_d
         q = ops.RelightParams().set(nodes=self.nodes, tris=self.tri, tri_ids=self.tri_ids, faces=self.faces, vmat=self.vmat_d, env=e['env'],
                                     env_p=e['p'], cdf_rows=e['cdf_rows'], cdf_cols=e['cdf_cols'], accum=accum, rays=self.rays)
@@ -509,6 +502,24 @@ class Relighter:
         q.K[:] = [K[0, 0], K[1, 1], K[0, 2], K[1, 2]]
         q.env_w, q.env_h, q.width, q.height = self.env_w, self.env_h, w, h
         q.max_bounces, q.ggx_smith, q.seed = max_bounces, self.ggx_smith, seed & 0xffffffff
+        return q
+
+    def render(self, pose, K, h, w, spp, max_bounces=4, seed=0, spp_per_launch=16, denoise=False):
+        """One image -> CUDA float32 [h,w,4]: linear RGB premultiplied by coverage, alpha = fraction of camera samples that hit
+        the mesh.  pose: world -> camera [3,4] (OpenCV axes), K: [3,3] pinhole intrinsics.  The samples are launched in
+        chunks of spp_per_launch; the result does not depend on the chunking.  self.rays accumulates the rays traced.
+        denoise=True traces with the feature buffers and returns the frame filtered by nero_b200.denoise.denoise (default
+        settings; focal K[0,0]) in the same layout, with the same alpha."""
+        import torch
+        from . import ops
+        if denoise:
+            from .denoise import denoise as run_denoise
+            accum, aov = self.render_sums(pose, K, h, w, spp, max_bounces, seed, spp_per_launch)
+            return run_denoise(accum, aov, spp, float(np.asarray(K, np.float64)[0, 0]))
+        if spp < 1 or max_bounces < 1 or spp_per_launch < 1:
+            raise ValueError('spp, max_bounces and spp_per_launch must be positive')
+        accum = torch.zeros(h * w, 4, device=self.dev)
+        q = self._params(pose, K, h, w, max_bounces, seed, accum)
         for s0 in range(0, spp, spp_per_launch):
             q.spp0, q.spp = s0, min(spp_per_launch, spp - s0)
             if self.uv is None:
@@ -517,3 +528,23 @@ class Relighter:
                 ops.K('nero_relight_render_textured', q, self.vt_d, self.ft_d, self.vt_d.shape[0], self.tex_d, self.tex.shape[1],
                       self.tex.shape[0])
         return (accum / spp).reshape(h, w, 4)
+
+    def render_sums(self, pose, K, h, w, spp, max_bounces=4, seed=0, spp_per_launch=16):
+        """The samples of render() traced by the AOV instances -> (accum [h,w,4], aov [h,w,16]) CUDA float32 sums over the
+        samples: accum holds the bits render() divides by spp, aov the denoiser's feature sums (include/nero_denoise.h)."""
+        import torch
+        from . import ops
+        from .denoise import AOV
+        if spp < 1 or max_bounces < 1 or spp_per_launch < 1:
+            raise ValueError('spp, max_bounces and spp_per_launch must be positive')
+        accum = torch.zeros(h * w, 4, device=self.dev)
+        aov = torch.zeros(h * w, AOV, device=self.dev)
+        q = self._params(pose, K, h, w, max_bounces, seed, accum)
+        for s0 in range(0, spp, spp_per_launch):
+            q.spp0, q.spp = s0, min(spp_per_launch, spp - s0)
+            if self.uv is None:
+                ops.K('nero_relight_render_aov', q, aov)
+            else:
+                ops.K('nero_relight_render_textured_aov', q, self.vt_d, self.ft_d, self.vt_d.shape[0], self.tex_d, self.tex.shape[1],
+                      self.tex.shape[0], aov)
+        return accum.reshape(h, w, 4), aov.reshape(h, w, AOV)

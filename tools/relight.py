@@ -10,6 +10,12 @@ textured OBJ of tools/extract_materials_texture_map.py with its MTL and feat{0,1
 Renders frames k = 0 .. num-1 of the reference's turntable (blender_backend/relight_backend.py) to data/relight/<name>/<k>.png
 (RGBA8, transparent background); frames that already exist are skipped.  The scene -- geometry, materials, BRDF, cameras,
 environment mapping and output encoding -- is stated in nero_b200/relight.py.  Paths are relative to the working directory.
+
+--denoise filters each frame with the feature-guided a-trous filter of nero_b200/denoise.py before it is written; frames,
+names and the PNG format are unchanged, and so is the alpha channel.  The intended use is `--samples 64 --denoise` in place of
+the default 1024 samples:
+
+    python tools/relight.py --mesh ... --material ... --hdr ... --name bell --samples 64 --denoise
 """
 import argparse
 import os
@@ -38,6 +44,7 @@ def parse(argv=None):
     parser.add_argument('--bounces', type=int, default=4)
     parser.add_argument('--geometry', choices=('schlick', 'ggx_smith'), default='schlick')
     parser.add_argument('--seed', type=int, default=0)
+    parser.add_argument('--denoise', action='store_true', default=False, help='denoise each frame (use with --samples 64)')
     flags = parser.parse_args(argv)
     if flags.obj is not None:
         if flags.mesh is not None or flags.material is not None:
@@ -73,7 +80,8 @@ def main(argv=None):
         path = os.path.join(out_dir, f'{k}.png')
         if os.path.exists(path):
             continue
-        img = relighter.render(poses[k], K, flags.height, flags.width, flags.samples, flags.bounces, flags.seed)
+        img = relighter.render(poses[k], K, flags.height, flags.width, flags.samples, flags.bounces, flags.seed,
+                               denoise=flags.denoise)
         torch.cuda.synchronize()
         write_png_rgba(path, to_rgba8(img.cpu().numpy()))
         print(path)
