@@ -27,6 +27,8 @@ extern "C" {
 int nero_relight_render_textured(const nero_relight_params* q, const float* vt, const int* ft, int n_uv, const float* tex, int tex_w,
                                  int tex_h, void* stream);
 
+/* The normal-mapped instances, nero_relight_render_textured_nmap and _nmap_aov, are declared in include/nero_normalmap.h. */
+
 #ifdef __cplusplus
 }
 #endif

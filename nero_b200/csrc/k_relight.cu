@@ -10,10 +10,15 @@
 // the power heuristic.  No Russian roulette: at most 1 + 2 * max_bounces rays per path.
 // The kAov instances also add each hitting sample's first-hit guides and demodulated radiance into the feature sums the
 // denoiser reads (include/nero_denoise.h); they only read values the colour path computes, so accum keeps its bits.
+// The normal-mapped source (NmapTexMaterials) also returns the flat normal next to the shading normal; the shading rule
+// that separates them is stated in include/nero_normalmap.h.  The other sources compile as if the rule did not exist.
+#include <type_traits>
+
 #include "bvh_traverse.cuh"
 #include "common.cuh"
 #include "math_relight.cuh"
 #include "../../include/nero_denoise.h"
+#include "../../include/nero_normalmap.h"
 #include "../../include/nero_relight_tex.h"
 
 namespace nero {
@@ -21,25 +26,32 @@ namespace nero {
 namespace {
 
 struct SurfHit {
-  float p[3], n[3];     // hit point, unit normal facing the incoming ray
+  float p[3], n[3];     // hit point, unit (shading) normal facing the incoming ray
   float albedo[3], metallic, alpha;
+  float ng[3];          // normal-mapped sources only: the flat normal facing the incoming ray (the others shade with it, as n)
 };
 
-// hit point and flat normal, shared by both material sources
-__device__ __forceinline__ void hit_geometry(const nero_relight_params& q, const BvhHit& h, const float* o, const float* d, SurfHit& s) {
+// hit point and flat normal, shared by every material source; returns the sign the outward normal was multiplied by
+__device__ __forceinline__ float hit_geometry(const nero_relight_params& q, const BvhHit& h, const float* o, const float* d, SurfHit& s) {
   const float4* tris = reinterpret_cast<const float4*>(q.tris);
   const float4 e1 = __ldg(tris + 3 * h.tri + 1), e2 = __ldg(tris + 3 * h.tri + 2);
   // marching-cubes meshes are wound with cross(e1, e2) pointing into the solid: the outward normal is its negation
   float n[3] = {-(e1.y * e2.z - e1.z * e2.y), -(e1.z * e2.x - e1.x * e2.z), -(e1.x * e2.y - e1.y * e2.x)};
   normalize3(n, n);
-  if (rl_dot(n, d) > 0.f) { n[0] = -n[0]; n[1] = -n[1]; n[2] = -n[2]; }   // two-sided
+  const bool flip = rl_dot(n, d) > 0.f;
+  if (flip) { n[0] = -n[0]; n[1] = -n[1]; n[2] = -n[2]; }   // two-sided
   for (int k = 0; k < 3; ++k) { s.p[k] = o[k] + h.t * d[k]; s.n[k] = n[k]; }
+  return flip ? -1.0f : 1.0f;
 }
 
 struct VertexMaterials {};          // q.vmat [V,8] rows, interpolated barycentrically
 struct TexMaterials {              // include/nero_relight_tex.h: vt [n_uv,2], ft [T,3], tex [h,w,8]
   const float2* vt; const int* ft; const float4* tex; int w, h;
 };
+struct NmapTexMaterials : TexMaterials {};   // the same arrays; texel channels 5-7 hold an object-space normal map
+
+template <class Materials>
+constexpr bool kNormalMapped = std::is_same<Materials, NmapTexMaterials>::value;
 
 __device__ __forceinline__ void surface(const nero_relight_params& q, VertexMaterials, const BvhHit& h, const float* o, const float* d,
                                         SurfHit& s) {
@@ -68,10 +80,12 @@ __device__ __forceinline__ int wrap(int i, int n) {   // positive modulo: the re
 
 // Textured materials: uv interpolated like the per-vertex rows, then a bilinear, wrapping fetch of the [h,w,8] texel rows with
 // v = 0 at the bottom image row (row h-1).  alpha is the filtered roughness itself: the texture export stores the rescaled
-// roughness NeRO's shading takes, not its square root.
-__device__ __forceinline__ void surface(const nero_relight_params& q, const TexMaterials& m, const BvhHit& h, const float* o,
-                                        const float* d, SurfHit& s) {
-  hit_geometry(q, h, o, d, s);
+// roughness NeRO's shading takes, not its square root.  kNmap: the texel's second float4 is loaded whole (roughness and the
+// map normal), the normal is filtered like the other channels and becomes the shading normal (include/nero_normalmap.h).
+template <bool kNmap>
+__device__ __forceinline__ void tex_surface(const nero_relight_params& q, const TexMaterials& m, const BvhHit& h, const float* o,
+                                            const float* d, SurfHit& s) {
+  const float sg = hit_geometry(q, h, o, d, s);
   const int f = __ldg(q.tri_ids + h.tri);
   const float w0 = 1.0f - h.u - h.v;
   float2 t[3];
@@ -85,11 +99,16 @@ __device__ __forceinline__ void surface(const nero_relight_params& q, const TexM
   const int ix1 = ix + 1 == m.w ? 0 : ix + 1, iy1 = iy + 1 == m.h ? 0 : iy + 1;
   const size_t r0 = size_t(iy) * m.w, r1 = size_t(iy1) * m.w;
   const size_t tap[4] = {r0 + ix, r0 + ix1, r1 + ix, r1 + ix1};
-  float4 a[4];
+  float4 a[4], nb[4];
   float r[4];
   for (int k = 0; k < 4; ++k) {
     a[k] = __ldg(m.tex + 2 * tap[k]);
-    r[k] = __ldg(reinterpret_cast<const float*>(m.tex + 2 * tap[k] + 1));
+    if constexpr (kNmap) {
+      nb[k] = __ldg(m.tex + 2 * tap[k] + 1);
+      r[k] = nb[k].x;
+    } else {
+      r[k] = __ldg(reinterpret_cast<const float*>(m.tex + 2 * tap[k] + 1));
+    }
   }
   auto lerp = [](float p, float q_, float w) { return p + w * (q_ - p); };
   auto bilerp = [&](float c00, float c10, float c01, float c11) { return lerp(lerp(c00, c10, fx), lerp(c01, c11, fx), fy); };
@@ -98,6 +117,30 @@ __device__ __forceinline__ void surface(const nero_relight_params& q, const TexM
   s.albedo[2] = bilerp(a[0].z, a[1].z, a[2].z, a[3].z);
   s.metallic = bilerp(a[0].w, a[1].w, a[2].w, a[3].w);
   s.alpha = bilerp(r[0], r[1], r[2], r[3]);
+  if constexpr (kNmap) {
+    float ns[3] = {bilerp(nb[0].y, nb[1].y, nb[2].y, nb[3].y), bilerp(nb[0].z, nb[1].z, nb[2].z, nb[3].z),
+                   bilerp(nb[0].w, nb[1].w, nb[2].w, nb[3].w)};
+    const float len = sqrtf(rl_dot(ns, ns));
+    bool use = len >= 1e-6f;
+    if (use) {
+      for (int k = 0; k < 3; ++k) ns[k] = sg * (ns[k] / len);   // flipped by the sign that made the flat normal face the ray
+      use = rl_dot(ns, d) < 0.f;                                 // dot(n_s, wo) > 0
+    }
+    for (int k = 0; k < 3; ++k) {
+      s.ng[k] = s.n[k];
+      if (use) s.n[k] = ns[k];
+    }
+  }
+}
+
+__device__ __forceinline__ void surface(const nero_relight_params& q, const TexMaterials& m, const BvhHit& h, const float* o,
+                                        const float* d, SurfHit& s) {
+  tex_surface<false>(q, m, h, o, d, s);
+}
+
+__device__ __forceinline__ void surface(const nero_relight_params& q, const NmapTexMaterials& m, const BvhHit& h, const float* o,
+                                        const float* d, SurfHit& s) {
+  tex_surface<true>(q, m, h, o, d, s);
 }
 
 __device__ __forceinline__ float mis(float a, float b) {   // power heuristic a^2 / (a^2 + b^2)
@@ -108,6 +151,7 @@ __device__ __forceinline__ float mis(float a, float b) {   // power heuristic a^
 template <class Materials, bool kAov>
 __global__ void __launch_bounds__(128) relight_kernel(const nero_relight_params q, const Materials mat, float4* aov) {
   const int x = blockIdx.x * 16 + (threadIdx.x & 15), y = blockIdx.y * 8 + (threadIdx.x >> 4);
+  constexpr bool kNmap = kNormalMapped<Materials>;
   if (x >= q.width || y >= q.height) return;
   const uint32_t pix = uint32_t(y) * uint32_t(q.width) + uint32_t(x);
   const float4* n4 = reinterpret_cast<const float4*>(q.nodes);
@@ -159,7 +203,7 @@ __global__ void __launch_bounds__(128) relight_kernel(const nero_relight_params 
       surface(q, mat, h, o, d, sh);
       const float v[3] = {-d[0], -d[1], -d[2]};
       float po[3];
-      for (int k = 0; k < 3; ++k) po[k] = sh.p[k] + kRelightEps * sh.n[k];
+      for (int k = 0; k < 3; ++k) po[k] = sh.p[k] + kRelightEps * (kNmap ? sh.ng[k] : sh.n[k]);   // offsets along the flat normal
       const uint32_t bb = uint32_t(b);
       const float ps = rl_spec_prob(sh.albedo, sh.metallic);
       // next-event estimation from the environment
@@ -172,7 +216,7 @@ __global__ void __launch_bounds__(128) relight_kernel(const nero_relight_params 
         const float ce = rl_env_dir(uu, vv, l);
         const float pl = rl_env_pdf(__ldg(q.env_p + size_t(j) * W + i), W, H, ce);
         const float NoL = rl_dot(sh.n, l);
-        if (NoL > 0.f && pl > 0.f) {
+        if (NoL > 0.f && pl > 0.f && (!kNmap || rl_dot(sh.ng, l) > 0.f)) {   // below the flat face: carries nothing
           float f[3];
           rl_brdf(sh.n, v, l, sh.albedo, sh.metallic, sh.alpha, q.ggx_smith, f);
           ++rays;
@@ -194,6 +238,7 @@ __global__ void __launch_bounds__(128) relight_kernel(const nero_relight_params 
       normalize3(l, l);
       const float pb = rl_bsdf_pdf(sh.n, v, l, sh.alpha, ps);
       if (!(pb > 0.f)) break;
+      if (kNmap && !(rl_dot(sh.ng, l) > 0.f)) break;   // a continuation below the flat face ends the path
       float f[3];
       rl_brdf(sh.n, v, l, sh.albedo, sh.metallic, sh.alpha, q.ggx_smith, f);
       const float NoL = rl_dot(sh.n, l);
@@ -268,6 +313,14 @@ extern "C" int nero_relight_render_textured(const nero_relight_params* p, const 
   return launch<false>(*p, m, nullptr, stream);
 }
 
+extern "C" int nero_relight_render_textured_nmap(const nero_relight_params* p, const float* vt, const int* ft, int n_uv,
+                                                 const float* tex, int tex_w, int tex_h, void* stream) {
+  if (!p || p->vmat || !scene_ok(*p) || !vt || !ft || !tex || n_uv < 1 || tex_w < 1 || tex_h < 1) return NERO_ERR_ARG;
+  NmapTexMaterials m;
+  m.vt = reinterpret_cast<const float2*>(vt); m.ft = ft; m.tex = reinterpret_cast<const float4*>(tex); m.w = tex_w; m.h = tex_h;
+  return launch<false>(*p, m, nullptr, stream);
+}
+
 extern "C" int nero_relight_render_aov(const nero_relight_params* p, float* aov, void* stream) {
   if (!p || !p->vmat || !scene_ok(*p) || !aov) return NERO_ERR_ARG;
   return launch<true>(*p, VertexMaterials{}, aov, stream);
@@ -277,6 +330,14 @@ extern "C" int nero_relight_render_textured_aov(const nero_relight_params* p, co
                                                 const float* tex, int tex_w, int tex_h, float* aov, void* stream) {
   if (!p || p->vmat || !scene_ok(*p) || !vt || !ft || !tex || n_uv < 1 || tex_w < 1 || tex_h < 1 || !aov) return NERO_ERR_ARG;
   const TexMaterials m{reinterpret_cast<const float2*>(vt), ft, reinterpret_cast<const float4*>(tex), tex_w, tex_h};
+  return launch<true>(*p, m, aov, stream);
+}
+
+extern "C" int nero_relight_render_textured_nmap_aov(const nero_relight_params* p, const float* vt, const int* ft, int n_uv,
+                                                     const float* tex, int tex_w, int tex_h, float* aov, void* stream) {
+  if (!p || p->vmat || !scene_ok(*p) || !vt || !ft || !tex || n_uv < 1 || tex_w < 1 || tex_h < 1 || !aov) return NERO_ERR_ARG;
+  NmapTexMaterials m;
+  m.vt = reinterpret_cast<const float2*>(vt); m.ft = ft; m.tex = reinterpret_cast<const float4*>(tex); m.w = tex_w; m.h = tex_h;
   return launch<true>(*p, m, aov, stream);
 }
 

@@ -5,7 +5,8 @@
 //              with the top-left rule (either winding; zero-area triangles own nothing).  owner = atomicMin(triangle id), so
 //              the map is deterministic even where triangles overlap; cover counts them.
 //   compact    ordered compaction of the covered texels in row-major order: count -> one-block scan -> emit
-//              (compact.cuh).  emit interpolates the mesh positions in fp32 with the barycentrics of the same edge functions.
+//              (compact.cuh).  emit interpolates the mesh positions in fp32 with the barycentrics of the same edge functions
+//              (texel_bary.cuh, shared with the normal-map bake).
 //   encode     linear_to_srgb in fp64 as numpy evaluates it (no contraction), x 255, truncated to uint8.
 //   inpaint    search texels (covered, Manhattan distance <= 3 from an uncovered texel or the border), a 16x16 tile map of
 //              them, then per uncovered texel a ring-by-ring scan of the radius-32 window for the nearest search texel.
@@ -15,6 +16,7 @@
 // run to run.
 #include "common.cuh"
 #include "compact.cuh"
+#include "texel_bary.cuh"
 #include "../../include/nero_texmap.h"
 
 namespace nero {
@@ -29,41 +31,6 @@ constexpr int kTile = 16;          // tile of the search-texel occupancy map
 __device__ __forceinline__ long long floordiv(long long a, long long b) {
   const long long q = a / b;
   return (a % b != 0 && ((a < 0) != (b < 0))) ? q - 1 : q;
-}
-
-// uv of triangle t snapped to 1/256 texel: round-half-even of u * width * 256 (exact in fp64)
-struct SnapTri {
-  long long x[3], y[3];
-  long long area;   // positive orientation after the sign s
-  int s;
-};
-
-__device__ __forceinline__ SnapTri snap_tri(const float* __restrict__ vt, const int* __restrict__ ft, int t, int width, int height) {
-  SnapTri q;
-  for (int i = 0; i < 3; ++i) {
-    const int k = __ldg(ft + 3 * t + i);
-    q.x[i] = llrint(double(__ldg(vt + 2 * k)) * double(width) * 256.0);
-    q.y[i] = llrint(double(__ldg(vt + 2 * k + 1)) * double(height) * 256.0);
-  }
-  const long long a = (q.x[1] - q.x[0]) * (q.y[2] - q.y[0]) - (q.y[1] - q.y[0]) * (q.x[2] - q.x[0]);
-  q.s = a < 0 ? -1 : 1;
-  q.area = a < 0 ? -a : a;
-  return q;
-}
-
-// edge weights w[i] (edge opposite vertex i) at the texel centre (px, py) in 1/256 texel; true if the texel is covered
-__device__ __forceinline__ bool tri_cover(const SnapTri& q, long long px, long long py, long long w[3]) {
-  bool in = true;
-#pragma unroll
-  for (int i = 0; i < 3; ++i) {
-    const int a = (i + 1) % 3, b = (i + 2) % 3;
-    const long long dx = q.x[b] - q.x[a], dy = q.y[b] - q.y[a];
-    w[i] = q.s * (dx * (py - q.y[a]) - dy * (px - q.x[a]));
-    const long long sdx = q.s * dx, sdy = q.s * dy;
-    const bool top_left = sdy < 0 || (sdy == 0 && sdx > 0);
-    in = in && (w[i] > 0 || (w[i] == 0 && top_left));
-  }
-  return in;
 }
 
 __global__ void __launch_bounds__(128) raster_kernel(const float* __restrict__ vt, const int* __restrict__ ft, int T, int width, int height,
@@ -122,22 +89,12 @@ __global__ void __launch_bounds__(kTxThreads) texel_emit_kernel(const unsigned* 
     int total;
     const int off = block_scan<kTxThreads>(keep ? 1 : 0, s_w, &total);
     if (keep) {
-      const int t = int(__ldg(owner + L));
-      const SnapTri q = snap_tri(vt, ft, t, width, height);
-      const long long y = L / width, x = L - y * width;
-      long long w[3];
-      tri_cover(q, 256 * x + 128, 256 * y + 128, w);
-      float b[3];
-#pragma unroll
-      for (int i = 0; i < 3; ++i) b[i] = float(double(w[i]) / double(q.area));
-      const float* p0 = verts + 3 * size_t(__ldg(faces + 3 * t));
-      const float* p1 = verts + 3 * size_t(__ldg(faces + 3 * t + 1));
-      const float* p2 = verts + 3 * size_t(__ldg(faces + 3 * t + 2));
+      float b[3], p[3];
+      texel_point(vt, ft, verts, faces, int(__ldg(owner + L)), L, width, height, b, p);
       const long long o = pbase + off;
       texel[o] = int(L);
 #pragma unroll
-      for (int k = 0; k < 3; ++k)
-        xyz[3 * o + k] = __fadd_rn(__fadd_rn(__fmul_rn(b[0], __ldg(p0 + k)), __fmul_rn(b[1], __ldg(p1 + k))), __fmul_rn(b[2], __ldg(p2 + k)));
+      for (int k = 0; k < 3; ++k) xyz[3 * o + k] = p[k];
     }
     pbase += total;
   }

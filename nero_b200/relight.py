@@ -105,14 +105,17 @@ def vertex_material_table(materials):
 class UVMaterials:
     """Materials as UV textures: vt [N,2] float uv, ft [T,3] int indices into vt (one row per triangle of the mesh), and
     linear (decoded) maps with row 0 at the top of the image: albedo [H,W,3], metallic [H,W] or [H,W,1], roughness [H,W] or
-    [H,W,1] (the rescaled roughness, the BRDF's alpha itself)."""
+    [H,W,1] (the rescaled roughness, the BRDF's alpha itself).  normal: an optional object-space normal map [H,W,3] the size of
+    the albedo map (nero_b200/normalmap.py: decoded linearly, outward unit normals in the mesh's coordinates); with it the
+    relighter shades with the map's normals (the rule of include/nero_normalmap.h)."""
 
-    def __init__(self, vt, ft, albedo, metallic, roughness):
+    def __init__(self, vt, ft, albedo, metallic, roughness, normal=None):
         self.vt = np.ascontiguousarray(vt, np.float32)
         self.ft = np.ascontiguousarray(ft, np.int32)
         self.albedo = np.asarray(albedo, np.float32)
         self.metallic = np.asarray(metallic, np.float32)
         self.roughness = np.asarray(roughness, np.float32)
+        self.normal = None if normal is None else np.asarray(normal, np.float32)
         if self.vt.ndim != 2 or self.vt.shape[1] != 2 or self.vt.shape[0] < 1:
             raise ValueError(f'vt has shape {self.vt.shape}; expected [N,2] with N >= 1')
         if self.ft.ndim != 2 or self.ft.shape[1] != 3:
@@ -126,15 +129,20 @@ class UVMaterials:
             a = getattr(self, k)
             if a.shape not in (hw, hw + (1,)):
                 raise ValueError(f'{k} map has shape {a.shape}; the albedo map is {hw}')
-        if not all(np.isfinite(a).all() for a in (self.vt, self.albedo, self.metallic, self.roughness)):
+        if self.normal is not None and self.normal.shape != hw + (3,):
+            raise ValueError(f'normal map has shape {self.normal.shape}; the albedo map is {hw}, so [{hw[0]},{hw[1]},3] is expected')
+        maps = (self.vt, self.albedo, self.metallic, self.roughness) + (() if self.normal is None else (self.normal,))
+        if not all(np.isfinite(a).all() for a in maps):
             raise ValueError('UV materials hold non-finite values')
 
     def texel_table(self):
-        """[H,W,8] float32 texel rows (albedo rgb, metallic, roughness, 0, 0, 0), the layout nero_relight_render_textured
-        reads."""
+        """[H,W,8] float32 texel rows (albedo rgb, metallic, roughness, then the normal map's xyz or 0, 0, 0), the layout
+        nero_relight_render_textured (and _nmap) reads."""
         H, W = self.albedo.shape[:2]
         t = np.zeros((H, W, 8), np.float32)
         t[..., :3], t[..., 3], t[..., 4] = self.albedo, self.metallic.reshape(H, W), self.roughness.reshape(H, W)
+        if self.normal is not None:
+            t[..., 5:] = self.normal
         return t
 
 
@@ -476,6 +484,7 @@ class Relighter:
             if self.uv.ft.shape != self.tris.shape:
                 raise ValueError(f'ft has shape {self.uv.ft.shape} for tris of shape {self.tris.shape}')
             self.vmat, self.vmat_d = None, None
+            self.nmap = self.uv.normal is not None
             self.tex = self.uv.texel_table()
             self.vt_d, self.ft_d, self.tex_d = up(self.uv.vt), up(self.uv.ft), up(self.tex)
         else:
@@ -525,7 +534,7 @@ class Relighter:
             if self.uv is None:
                 ops.K('nero_relight_render', q)
             else:
-                ops.K('nero_relight_render_textured', q, self.vt_d, self.ft_d, self.vt_d.shape[0], self.tex_d, self.tex.shape[1],
+                ops.K('nero_relight_render_textured_nmap' if self.nmap else 'nero_relight_render_textured', q, self.vt_d, self.ft_d, self.vt_d.shape[0], self.tex_d, self.tex.shape[1],
                       self.tex.shape[0])
         return (accum / spp).reshape(h, w, 4)
 
@@ -545,6 +554,6 @@ class Relighter:
             if self.uv is None:
                 ops.K('nero_relight_render_aov', q, aov)
             else:
-                ops.K('nero_relight_render_textured_aov', q, self.vt_d, self.ft_d, self.vt_d.shape[0], self.tex_d, self.tex.shape[1],
+                ops.K('nero_relight_render_textured_nmap_aov' if self.nmap else 'nero_relight_render_textured_aov', q, self.vt_d, self.ft_d, self.vt_d.shape[0], self.tex_d, self.tex.shape[1],
                       self.tex.shape[0], aov)
         return accum.reshape(h, w, 4), aov.reshape(h, w, AOV)

@@ -16,6 +16,12 @@ names and the PNG format are unchanged, and so is the alpha channel.  The intend
 the default 1024 samples:
 
     python tools/relight.py --mesh ... --material ... --hdr ... --name bell --samples 64 --denoise
+
+--normal-map (with --obj) shades with an object-space normal map baked onto the OBJ's atlas by tools/bake_normal_map.py,
+so a simplified mesh renders with its fine mesh's normals.  The map must be the size of the albedo map; with --trans it is
+rotated with the mesh.  Without --normal-map the frames are those of the textured materials alone:
+
+    python tools/relight.py --obj n2m/mesh_0.obj --normal-map n2m/normal_0.png --hdr ... --name bell
 """
 import argparse
 import os
@@ -45,7 +51,11 @@ def parse(argv=None):
     parser.add_argument('--geometry', choices=('schlick', 'ggx_smith'), default='schlick')
     parser.add_argument('--seed', type=int, default=0)
     parser.add_argument('--denoise', action='store_true', default=False, help='denoise each frame (use with --samples 64)')
+    parser.add_argument('--normal-map', type=str, default=None,
+                        help='object-space normal map of the --obj mesh (tools/bake_normal_map.py writes normal_0.png)')
     flags = parser.parse_args(argv)
+    if flags.normal_map is not None and flags.obj is None:
+        parser.error('--normal-map needs --obj (the map belongs to the textured OBJ\'s atlas)')
     if flags.obj is not None:
         if flags.mesh is not None or flags.material is not None:
             parser.error('--obj cannot be combined with --mesh / --material')
@@ -65,7 +75,17 @@ def main(argv=None):
 
     if flags.obj is not None:
         verts, tris, vt, ft, maps = load_textured_obj(flags.obj)
-        materials = UVMaterials(vt, ft, maps['albedo'], maps['metallic'], maps['roughness'])
+        normal = None
+        if flags.normal_map is not None:
+            from nero_b200.normalmap import read_normal_map
+            normal = read_normal_map(flags.normal_map)
+            (h, w), (ha, wa) = normal.shape[:2], maps['albedo'].shape[:2]
+            if (h, w) != (ha, wa):
+                raise SystemExit(f'relight.py: error: {flags.normal_map}: the normal map is {w}x{h} but the albedo map of '
+                                 f'{flags.obj} is {wa}x{ha}; bake it with --size {ha}')
+            if flags.trans:
+                normal = (normal.astype(np.float64) @ MESH_TRANS.T).astype(np.float32)
+        materials = UVMaterials(vt, ft, maps['albedo'], maps['metallic'], maps['roughness'], normal=normal)
     else:
         verts, tris = read_ply(flags.mesh)
         materials = load_materials(flags.material)
