@@ -1,5 +1,6 @@
-// The texel -> surface point map of the UV atlas, shared by the texture export (k_texmap.cu: raster and texel_emit) and the
-// normal-map bake (k_normalmap.cu), so a bake point is the point the export stores in raster()['xyz'], bit for bit.
+// The texel -> surface point map of the UV atlas, shared by the texture export (k_texmap.cu: raster and texel_emit), the
+// normal-map bake (k_normalmap.cu) and the glTF export's tangent-space conversion (k_gltf.cu), so a bake point is the point
+// the export stores in raster()['xyz'], bit for bit.
 //
 // uv is snapped to 1/256 texel (round-half-even of u * width * 256, exact in fp64); coverage uses exact int64 edge functions
 // with the top-left rule for either winding; the barycentrics of a covered texel are w_i / area rounded once to fp32, and
@@ -44,16 +45,22 @@ __device__ __forceinline__ bool tri_cover(const SnapTri& q, long long px, long l
   return in;
 }
 
-// barycentrics b [3] and position p [3] of texel L (row-major in a width-wide atlas) owned by triangle t
-__device__ __forceinline__ void texel_point(const float* __restrict__ vt, const int* __restrict__ ft, const float* __restrict__ verts,
-                                            const int* __restrict__ faces, int t, long long L, int width, int height, float b[3],
-                                            float p[3]) {
+// barycentrics b [3] of texel L (row-major in a width-wide atlas) owned by triangle t
+__device__ __forceinline__ void texel_bary(const float* __restrict__ vt, const int* __restrict__ ft, int t, long long L, int width,
+                                           int height, float b[3]) {
   const SnapTri q = snap_tri(vt, ft, t, width, height);
   const long long y = L / width, x = L - y * width;
   long long w[3];
   tri_cover(q, 256 * x + 128, 256 * y + 128, w);
 #pragma unroll
   for (int i = 0; i < 3; ++i) b[i] = float(double(w[i]) / double(q.area));
+}
+
+// barycentrics b [3] and position p [3] of texel L owned by triangle t
+__device__ __forceinline__ void texel_point(const float* __restrict__ vt, const int* __restrict__ ft, const float* __restrict__ verts,
+                                            const int* __restrict__ faces, int t, long long L, int width, int height, float b[3],
+                                            float p[3]) {
+  texel_bary(vt, ft, t, L, width, height, b);
   const float* p0 = verts + 3 * size_t(__ldg(faces + 3 * t));
   const float* p1 = verts + 3 * size_t(__ldg(faces + 3 * t + 1));
   const float* p2 = verts + 3 * size_t(__ldg(faces + 3 * t + 2));

@@ -11,7 +11,8 @@ Convention
   * Object-space maps: a texel holds the outward unit normal in the OBJ's own coordinates, the coordinates the relighter
     renders in (tools/relight.py --trans rotates the map with the mesh).  Object space, because the relighter shades flat
     faces and an object-space map leaves no tangent-basis convention for the bake and the renderer to disagree on.
-    Tangent-space maps (MikkTSpace) are not supported.
+    The bake writes no tangent-space map; nero_b200/gltf.py (tools/export_gltf.py) converts this map to tangent space
+    against the tangents it writes into a glTF 2.0 file.
   * Outward normals.  Marching-cubes meshes are wound with cross(e1, e2) pointing into the solid, so outward is
     -cross(e1, e2); simplified meshes keep that winding.
   * Encoding per channel: k = floor((n 0.5 + 0.5) 255 + 0.5) clamped to [0, 255]; decoding is linear, 2k/255 - 1, with no
@@ -168,6 +169,11 @@ def write_normal_map(path, img):
 def read_normal_map(path):
     """An 8-bit RGB(A) normal-map image -> float32 [H,W,3] 2k/255 - 1 per channel (linear, not renormalised), row 0 the top
     row of the file.  A missing file, an unreadable one or one that is not 8-bit colour raises ValueError naming it."""
+    return decode(read_normal_map_bytes(path))
+
+
+def read_normal_map_bytes(path):
+    """read_normal_map's image as its uint8 RGB bytes [H,W,3], with the same checks."""
     import cv2
     if not os.path.isfile(path):
         raise ValueError(f'{path}: normal map file is missing')
@@ -176,4 +182,4 @@ def read_normal_map(path):
         raise ValueError(f'{path}: not an image OpenCV can read')
     if img.dtype != np.uint8 or img.ndim != 3 or img.shape[2] not in (3, 4):
         raise ValueError(f'{path}: a normal map must be an 8-bit RGB image, got {img.dtype} with shape {img.shape}')
-    return decode(img[..., [2, 1, 0]])
+    return np.ascontiguousarray(img[..., [2, 1, 0]])

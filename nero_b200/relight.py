@@ -183,6 +183,18 @@ def load_textured_obj(path):
     decoded with srgb_to_linear(k / 255), as load_materials decodes its arrays.  Anything else raises ValueError naming the
     file: faces that are not triangles or lack uv indices, indices out of range, non-finite values, a missing MTL or texture
     file, or maps of different sizes."""
+    V, tris, vt, ft, files = textured_obj_files(path)
+    maps = {k: _read_map(files[k], (0, 1, 2) if k == 'albedo' else (0,)) for k in MATERIAL_NAMES}
+    sizes = {k: m.shape[:2] for k, m in maps.items()}
+    if len(set(sizes.values())) != 1:
+        raise ValueError(f'{path}: texture maps differ in size: ' + ', '.join(f'{files[k]} {sizes[k][1]}x{sizes[k][0]}' for k in MATERIAL_NAMES))
+    return V, tris, vt, ft, maps
+
+
+def textured_obj_files(path):
+    """The geometry of load_textured_obj's OBJ and the paths of its texture files, checked as load_textured_obj checks them,
+    without reading the images -> (verts, tris, vt, ft as load_textured_obj returns them, {'albedo', 'metallic', 'roughness':
+    path})."""
     verts, uvs, faces, mtllib = [], [], [], None
     with open(path) as f:
         lines = f.read().splitlines()
@@ -244,11 +256,7 @@ def load_textured_obj(path):
     base = os.path.join(os.path.dirname(mtl_path), os.path.dirname(map_kd))
     files = {'albedo': os.path.join(base, name), 'metallic': os.path.join(base, name.replace('feat0_', 'feat1_', 1)),
              'roughness': os.path.join(base, name.replace('feat0_', 'feat2_', 1))}
-    maps = {k: _read_map(files[k], (0, 1, 2) if k == 'albedo' else (0,)) for k in MATERIAL_NAMES}
-    sizes = {k: m.shape[:2] for k, m in maps.items()}
-    if len(set(sizes.values())) != 1:
-        raise ValueError(f'{path}: texture maps differ in size: ' + ', '.join(f'{files[k]} {sizes[k][1]}x{sizes[k][0]}' for k in MATERIAL_NAMES))
-    return V.astype(np.float32), tris, N.astype(np.float32), ft, maps
+    return V.astype(np.float32), tris, N.astype(np.float32), ft, files
 
 
 # ------------------------------------------------------------------------------------------------ environment maps
@@ -440,6 +448,14 @@ def to_rgba8(img):
 
 def write_png(path, img):
     """Write uint8 [h,w,3] or [h,w,4] as an 8-bit RGB or RGBA PNG (stdlib zlib; no image library needed)."""
+    data = png_bytes(img)
+    with open(path, 'wb') as f:
+        f.write(data)
+
+
+def png_bytes(img):
+    """uint8 [h,w,3] or [h,w,4] -> the bytes of an 8-bit RGB or RGBA PNG: one IDAT chunk, filter type 0 on every row, zlib
+    level 6."""
     img = np.ascontiguousarray(img, np.uint8)
     if img.ndim != 3 or img.shape[2] not in (3, 4):
         raise ValueError(f'expected [h,w,3] or [h,w,4] uint8, got {img.shape}')
@@ -448,9 +464,8 @@ def write_png(path, img):
 
     def chunk(tag, body):
         return struct.pack('>I', len(body)) + tag + body + struct.pack('>I', zlib.crc32(tag + body) & 0xffffffff)
-    with open(path, 'wb') as f:
-        f.write(b'\x89PNG\r\n\x1a\n' + chunk(b'IHDR', struct.pack('>IIBBBBB', w, h, 8, 6 if c == 4 else 2, 0, 0, 0)) +
-                chunk(b'IDAT', zlib.compress(raw, 6)) + chunk(b'IEND', b''))
+    return (b'\x89PNG\r\n\x1a\n' + chunk(b'IHDR', struct.pack('>IIBBBBB', w, h, 8, 6 if c == 4 else 2, 0, 0, 0)) +
+            chunk(b'IDAT', zlib.compress(raw, 6)) + chunk(b'IEND', b''))
 
 
 def write_png_rgba(path, rgba):
