@@ -6,8 +6,9 @@ F, a GGX D (math_relight.cuh:rl_brdf), with glTF's roughness = sqrt(alpha).  So 
 changing its meaning.
 
 Input: the directory of tools/extract_materials_texture_map.py (mesh_0.obj, mesh_0.mtl, feat{0,1,2}_0.png, or the
-reference's JPEGs) as relight.load_textured_obj reads it, and optionally the object-space normal map of
-tools/bake_normal_map.py (normal_0.png, nero_b200/normalmap.py's convention).
+reference's JPEGs) as relight.load_textured_obj reads it, optionally the object-space normal map of
+tools/bake_normal_map.py (normal_0.png, nero_b200/normalmap.py's convention) and optionally the ambient-occlusion map of
+tools/bake_occlusion.py (occlusion_0.png, nero_b200/occlusion.py's convention).
 
 The file:
   * One scene, one node, one mesh, one triangle primitive.  Attributes POSITION (float32 with min / max), NORMAL, TEXCOORD_0
@@ -23,7 +24,9 @@ The file:
   * One material: baseColorTexture = feat0's bytes (both sRGB), metallicRoughnessTexture = (255, roughness, metallic) from
     feat1 / feat2 through the tables of include/nero_gltf.h (stored alpha -> sqrt, sRGB -> linear), factors 1; with a normal
     map, normalTexture = the map converted to tangent space against the file's own TANGENT and NORMAL, then seam-inpainted
-    with texmap.inpaint.  Images are PNGs (relight.png_bytes) in bufferViews; one sampler: LINEAR, LINEAR_MIPMAP_LINEAR,
+    with texmap.inpaint.  With an occlusion map, the metallic-roughness texture's red channel is the map's byte instead of
+    255 (glTF's "ORM" packing) and occlusionTexture = that same texture (index 1, strength 1 by default); G and B are
+    unchanged.  Without one the file is byte for byte what it is without the option.  Images are PNGs (relight.png_bytes) in bufferViews; one sampler: LINEAR, LINEAR_MIPMAP_LINEAR,
     REPEAT.
   * GLB container: JSON chunk padded with spaces, BIN chunk with zeros, every bufferView 4-byte aligned.
 
@@ -128,11 +131,12 @@ def metal_rough_cuda(metallic, roughness):
     return out
 
 
-def export_arrays(verts, tris, vt, ft, albedo, metallic, roughness, omap=None, profile=None):
+def export_arrays(verts, tris, vt, ft, albedo, metallic, roughness, omap=None, profile=None, occlusion=None):
     """The GPU stages of the export -> dict of numpy arrays: positions, normals, texcoords, tangents (None without omap),
     indices [T,3] uint32 (glTF's winding), images {base_color, metallic_roughness, normal (without omap: absent)}, and wv, wt,
     wf, covered (texels of the conversion, 0 without omap).  verts, tris, vt (the file's), ft as load_textured_obj returns
-    them; albedo [h,w,3], metallic / roughness [h,w] uint8 (the files' bytes); omap uint8 [h',w',3] (an object-space map).
+    them; albedo [h,w,3], metallic / roughness [h,w] uint8 (the files' bytes); omap uint8 [h',w',3] (an object-space map);
+    occlusion uint8 [h,w] (an ambient-occlusion map of the material maps' size, stored in metallic_roughness's red channel).
     profile (a dict) gets host-clock milliseconds of the phases normals / weld / tangents / tangent_space / metal_rough, each
     ended by a device synchronise."""
     import torch
@@ -148,6 +152,12 @@ def export_arrays(verts, tris, vt, ft, albedo, metallic, roughness, omap=None, p
     V = verts.shape[0]
     if tris.min() < 0 or tris.max() >= V or ft.min() < 0 or ft.max() >= vt.shape[0]:
         raise ValueError('export: triangle or uv indices out of range')
+    if occlusion is not None:
+        occlusion = np.asarray(occlusion, np.uint8)
+        mh, mw = np.asarray(metallic).shape[:2]
+        if occlusion.shape != (mh, mw):
+            raise ValueError(f'the occlusion map is {occlusion.shape[1]}x{occlusion.shape[0]} but the material maps are {mw}x{mh}'
+                             if occlusion.ndim == 2 else f'the occlusion map must be [h,w] uint8, got {occlusion.shape}')
     clock = [time.perf_counter()]
 
     def lap(phase):
@@ -176,6 +186,8 @@ def export_arrays(verts, tris, vt, ft, albedo, metallic, roughness, omap=None, p
         images['normal'] = inpaint(c['img'], c['raster']['owner'])[0][..., :3].cpu().numpy()
         lap('tangent_space')
     images['metallic_roughness'] = metal_rough_cuda(metallic, roughness).cpu().numpy()
+    if occlusion is not None:
+        images['metallic_roughness'][..., 0] = occlusion
     lap('metal_rough')
     wv, wt, wf = wv.cpu().numpy(), wt.cpu().numpy(), wf.cpu().numpy()
     uv = vt[wt]
@@ -189,11 +201,12 @@ def _pad4(n):
     return (4 - n % 4) % 4
 
 
-def glb_bytes(positions, normals, texcoords, indices, images, tangents=None, rotation=None):
+def glb_bytes(positions, normals, texcoords, indices, images, tangents=None, rotation=None, occlusion=False):
     """The GLB file of the module docstring -> bytes.  positions / normals [W,3], texcoords [W,2], tangents [W,4] float32 or
     None, indices [T,3] (written as uint32, already in glTF's winding), images {'base_color', 'metallic_roughness' and
-    optionally 'normal': uint8 [h,w,3]}, rotation a node quaternion [x,y,z,w] or None (identity).  Deterministic: the same
-    arrays give the same bytes."""
+    optionally 'normal': uint8 [h,w,3]}, rotation a node quaternion [x,y,z,w] or None (identity).  occlusion: the
+    metallic-roughness texture's red channel holds ambient occlusion, so the material also names it as its
+    occlusionTexture.  Deterministic: the same arrays give the same bytes."""
     from .relight import png_bytes
     arrays = {'positions': np.ascontiguousarray(positions, np.float32), 'normals': np.ascontiguousarray(normals, np.float32),
               'texcoords': np.ascontiguousarray(texcoords, np.float32)}
@@ -246,6 +259,8 @@ def glb_bytes(positions, normals, texcoords, indices, images, tangents=None, rot
     material = {'name': 'defaultMat', 'pbrMetallicRoughness': pbr}
     if 'normal' in images:
         material['normalTexture'] = {'index': 2}
+    if occlusion:
+        material['occlusionTexture'] = {'index': 1}
     node = {'mesh': 0}
     if rotation is not None:
         node['rotation'] = [float(x) for x in rotation]
@@ -262,9 +277,10 @@ def glb_bytes(positions, normals, texcoords, indices, images, tangents=None, rot
             struct.pack('<II', len(blob), _CHUNK_BIN) + bytes(blob))
 
 
-def export(obj_path, normal_map_path=None, trans=False, profile=None, stats=None):
-    """The .glb of the textured OBJ at obj_path (and the object-space normal map at normal_map_path) -> bytes.  trans: the
-    object is stored as tools/relight.py --trans takes it, so the node is not rotated.  profile (a dict) gets host-clock
+def export(obj_path, normal_map_path=None, trans=False, profile=None, stats=None, occlusion_path=None):
+    """The .glb of the textured OBJ at obj_path (and the object-space normal map at normal_map_path, and the ambient-occlusion
+    map at occlusion_path) -> bytes.  trans: the object is stored as tools/relight.py --trans takes it, so the node is not
+    rotated.  profile (a dict) gets host-clock
     milliseconds of the phases read / normals / weld / tangents / tangent_space / metal_rough / container; stats (a dict) gets
     positions, welded, triangles, covered."""
     import cv2
@@ -282,12 +298,19 @@ def export(obj_path, normal_map_path=None, trans=False, profile=None, stats=None
     if len(set(sizes.values())) != 1:
         raise ValueError(f'{obj_path}: texture maps differ in size: ' + ', '.join(f'{files[k]} {s[1]}x{s[0]}' for k, s in sizes.items()))
     omap = None if normal_map_path is None else read_normal_map_bytes(normal_map_path)
+    occ = None
+    if occlusion_path is not None:
+        from .occlusion import read_occlusion_map
+        occ = read_occlusion_map(occlusion_path)
+        (mh, mw), (oh, ow) = imgs['metallic'].shape[:2], occ.shape
+        if (oh, ow) != (mh, mw):
+            raise ValueError(f'{occlusion_path}: the occlusion map is {ow}x{oh} but the material maps are {mw}x{mh}')
     if profile is not None:
         profile['read'] = (time.perf_counter() - t0) * 1e3
-    out = export_arrays(verts, tris, vt, ft, imgs['albedo'], imgs['metallic'][..., 0], imgs['roughness'][..., 0], omap, profile)
+    out = export_arrays(verts, tris, vt, ft, imgs['albedo'], imgs['metallic'][..., 0], imgs['roughness'][..., 0], omap, profile, occ)
     t1 = time.perf_counter()
     data = glb_bytes(out['positions'], out['normals'], out['texcoords'], out['indices'], out['images'], out['tangents'],
-                     None if trans else Z_UP_ROTATION)
+                     None if trans else Z_UP_ROTATION, occ is not None)
     if profile is not None:
         profile['container'] = (time.perf_counter() - t1) * 1e3
     if stats is not None:
@@ -329,7 +352,8 @@ def _png_decode(data):
 def read_glb(path):
     """Read a .glb of this exporter's subset (a path or the bytes) -> dict json (the parsed JSON), positions, normals,
     texcoords, tangents (or None) float32, indices [T,3] uint32, rotation (or None), images {base_color, metallic_roughness[,
-    normal]: uint8 [h,w,3]}.  Anything outside the subset raises ValueError: another container version, chunk layout, more
+    normal]: uint8 [h,w,3]}, occlusion (the red channel [h,w] uint8 of the occlusionTexture's image, or None) and
+    occlusion_strength (its strength, 1.0 when not given, or None).  Anything outside the subset raises ValueError: another container version, chunk layout, more
     than one buffer / mesh / primitive, attributes other than this exporter's, component types, strides, sparse accessors,
     unaligned views or images that are not this exporter's PNGs."""
     data = path if isinstance(path, (bytes, bytearray)) else open(path, 'rb').read()
@@ -402,4 +426,12 @@ def read_glb(path):
         if img.get('mimeType') != 'image/png' or 'bufferView' not in img:
             raise ValueError(f'{key} image is not a PNG held in a bufferView')
         out['images'][key] = _png_decode(view_bytes(img['bufferView']))
+    occ = mats[0].get('occlusionTexture')
+    out['occlusion'], out['occlusion_strength'] = None, None
+    if occ is not None:
+        img = doc['images'][doc['textures'][occ['index']]['source']]
+        if img.get('mimeType') != 'image/png' or 'bufferView' not in img:
+            raise ValueError('occlusion image is not a PNG held in a bufferView')
+        out['occlusion'] = _png_decode(view_bytes(img['bufferView']))[..., 0].copy()
+        out['occlusion_strength'] = float(occ.get('strength', 1.0))
     return out

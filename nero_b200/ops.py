@@ -30,6 +30,7 @@ _SIMPLIFY_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_simplif
 _DENOISE_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_denoise.h')  # same library, plain-argument entry points
 _NORMALMAP_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_normalmap.h')  # same library, plain-argument entry points
 _GLTF_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_gltf.h')  # same library, plain-argument entry points
+_OCCLUSION_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_occlusion.h')  # same library, plain-argument entry points
 
 ACT_NONE, ACT_SOFTPLUS100, ACT_RELU, ACT_SIGMOID, ACT_EXPCLAMP = 0, 1, 2, 3, 4
 EPI_BIAS_ACT, EPI_MUL_DACT, EPI_TANGENT = 0, 1, 2
@@ -128,11 +129,13 @@ SIMPLIFY_PROTOS = _parse_header(_SIMPLIFY_HEADER)[1]
 DENOISE_PROTOS = _parse_header(_DENOISE_HEADER)[1]
 NORMALMAP_PROTOS = _parse_header(_NORMALMAP_HEADER)[1]
 GLTF_PROTOS = _parse_header(_GLTF_HEADER)[1]
+OCCLUSION_PROTOS = _parse_header(_OCCLUSION_HEADER)[1]
 for _name, _argtypes in (list(_PROTOS.items()) + list(TEXMAP_PROTOS.items()) + list(ENVMAP_PROTOS.items()) +
                          list(METRICS_PROTOS.items()) + list(RELIGHT_TEX_PROTOS.items()) + list(MESHPTS_PROTOS.items()) +
                          list(OBJPREP_PROTOS.items()) + list(MCSPARSE_PROTOS.items()) + list(MVS_PROTOS.items()) +
                          list(FEATURES_PROTOS.items()) + list(SFM_PROTOS.items()) + list(SIMPLIFY_PROTOS.items()) +
-                         list(DENOISE_PROTOS.items()) + list(NORMALMAP_PROTOS.items()) + list(GLTF_PROTOS.items())):
+                         list(DENOISE_PROTOS.items()) + list(NORMALMAP_PROTOS.items()) + list(GLTF_PROTOS.items()) +
+                         list(OCCLUSION_PROTOS.items())):
     _fn = getattr(lib, _name)
     _fn.argtypes, _fn.restype = _argtypes, ctypes.c_int
 # nero_abi_sizeof(i) is the size of ABI_RECORDS[i]; a library built from another version of the header would read the
