@@ -53,7 +53,7 @@ int nero_features_extrema(const float* dog, int w, int h, int levels, float thre
 /* Quadratic refinement in fp64 of n candidates cand [n,3] of octave `octave` (dog [levels, h, w]): at most 5 moves of one
  * sample each; a candidate is kept (ok = 1) when its last offset is below 1.5 in each coordinate, its refined |D| is
  * >= peak and tr(H)^2 / det(H) < (edge + 1)^2 / edge with det(H) > 0.  sigma = sigma0 2^(scale / (levels - 2)).  Writes
- * kp [n, NERO_FEATURES_KP]. */
+ * kp [n, NERO_FEATURES_KP]; cand and kp may be NULL when n = 0 (an octave without extrema). */
 int nero_features_refine(const float* dog, int w, int h, int levels, const int* cand, int n, int octave, double sigma0,
                          double peak, double edge, float* kp, void* stream);
 

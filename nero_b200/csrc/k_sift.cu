@@ -361,7 +361,7 @@ int nero_features_extrema(const float* dog, int w, int h, int levels, float thre
 
 int nero_features_refine(const float* dog, int w, int h, int levels, const int* cand, int n, int octave, double sigma0,
                          double peak, double edge, float* kp, void* stream) {
-  if (!dog || !kp || (n > 0 && !cand) || n < 0 || w < 2 * kBorder + 1 || h < 2 * kBorder + 1 || levels < 3 || octave < 0 ||
+  if (!dog || (n > 0 && (!cand || !kp)) || n < 0 || w < 2 * kBorder + 1 || h < 2 * kBorder + 1 || levels < 3 || octave < 0 ||
       octave >= NERO_FEATURES_MAX_OCTAVES || !(sigma0 > 0.0) || !(peak >= 0.0) || !(edge > 0.0))
     return NERO_ERR_ARG;
   if (n == 0) return NERO_OK;

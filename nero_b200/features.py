@@ -12,7 +12,9 @@ The protocol (k_sift.cu, k_match.cu, k_verify.cu, include/nero_features.h):
   * Images.  The files matching *.jpg, *.png, *.PNG, *.JPG of the image directory (in that pattern order, then sorted
     by path) get image ids 1..n.  Pixels are read in their stored order (mvs.read_rgb ignores an EXIF orientation), as
     run_colmap.py's skimage reader and COLMAP read them, so sizes, cameras and keypoints share COLMAP's frame.  Each image gets the camera SIMPLE_PINHOLE (f, w / 2, h / 2) with f = sqrt(w^2 + h^2)
-    and prior_focal_length = 1; with same_camera the first image's camera (id 1) serves every image.
+    and prior_focal_length = 1; with same_camera the first image's camera (id 1) serves every image.  With
+    camera_model='SIMPLE_RADIAL' the camera is SIMPLE_RADIAL (f, w / 2, h / 2, 0) with the same prior, for a mapper that
+    estimates k (COLMAP's); undistort.py then resamples the images.
   * Grey image.  mvs.prepare_grey (nero_mvs_grey) with s = ceil(max(w, h) / max_size): integer luma block-averaged over
     s x s.  Grey pixel p has its centre at image point (p + 1/2) s.
   * Scale space.  OCTAVES octaves of SCALES + 3 Gaussian levels; octave 0 is the grey image itself (COLMAP upsamples
@@ -85,6 +87,8 @@ MATCH_ROWS = 1 << 26     # row-best records (12 B each) per matcher launch
 _INT32_MAX = 2 ** 31 - 1
 PATTERNS = ('*.jpg', '*.png', '*.PNG', '*.JPG')
 SIMPLE_PINHOLE = 0
+SIMPLE_RADIAL = 2
+CAMERA_MODELS = {'SIMPLE_PINHOLE': SIMPLE_PINHOLE, 'SIMPLE_RADIAL': SIMPLE_RADIAL}   # the models the database may get
 UNCALIBRATED = 3
 MAX_IMAGE_ID = 2147483647
 
@@ -151,31 +155,34 @@ def image_size(path):
     return w, h
 
 
-def image_table(image_dir, same_camera=False):
+def image_table(image_dir, same_camera=False, camera_model='SIMPLE_PINHOLE'):
     """(names, cameras, camera id of each image) of an image directory, in id order."""
     if not os.path.isdir(image_dir):
         raise FileNotFoundError(f'{image_dir}: no image directory')
     names = list_images(image_dir)
     if not names:
         raise FileNotFoundError(f'{image_dir}: no *.jpg / *.png images')
-    cams, cam_of = cameras_for([image_size(os.path.join(image_dir, n)) for n in names], same_camera)
+    cams, cam_of = cameras_for([image_size(os.path.join(image_dir, n)) for n in names], same_camera, camera_model)
     return names, cams, cam_of
 
 
-def cameras_for(sizes, same_camera=False):
+def cameras_for(sizes, same_camera=False, camera_model='SIMPLE_PINHOLE'):
     """(cameras, images camera ids) for images of sizes [(w, h)] in id order: camera rows (camera_id, model, width, height,
-    params fp64, prior_focal_length)."""
+    params fp64, prior_focal_length).  camera_model: 'SIMPLE_PINHOLE' (f, cx, cy) or 'SIMPLE_RADIAL' (f, cx, cy, k = 0)."""
+    if camera_model not in CAMERA_MODELS:
+        raise ValueError(f'camera model {camera_model!r}: the database takes SIMPLE_PINHOLE or SIMPLE_RADIAL')
+    model, extra = CAMERA_MODELS[camera_model], [0.0] if camera_model == 'SIMPLE_RADIAL' else []
     cams, cam_of = [], []
     for k, (w, h) in enumerate(sizes):
         if not same_camera or k == 0:
             focal = np.sqrt(h ** 2 + w ** 2)
-            cams.append((len(cams) + 1, SIMPLE_PINHOLE, int(w), int(h), np.array([focal, w / 2, h / 2], np.float64), 1))
+            cams.append((len(cams) + 1, model, int(w), int(h), np.array([focal, w / 2, h / 2] + extra, np.float64), 1))
         cam_of.append(len(cams))
     return cams, cam_of
 
 
 def camera_K(cam):
-    f, cx, cy = cam[4]
+    f, cx, cy = cam[4][:3]
     return np.array([[f, 0, cx], [0, f, cy], [0, 0, 1]], np.float64)
 
 
@@ -455,10 +462,12 @@ def verify(points, hypotheses=HYPOTHESES, max_error=MAX_ERROR, seed=SEED):
     return F[:P].cpu().numpy(), best[:P].cpu().numpy(), count[:P].cpu().numpy(), [inl[off[k]:off[k + 1]] for k in range(P)]
 
 
-def build_database(image_dir, db_path, same_camera=False, max_size=MAX_SIZE, max_features=MAX_FEATURES, log=None):
-    """The whole tool: features of every image, all-pair matches and verified geometries written to db_path.  -> info."""
+def build_database(image_dir, db_path, same_camera=False, max_size=MAX_SIZE, max_features=MAX_FEATURES, log=None,
+                   camera_model='SIMPLE_PINHOLE'):
+    """The whole tool: features of every image, all-pair matches and verified geometries written to db_path.  -> info.
+    Two-view verification fits F on the raw keypoints whatever the camera model."""
     import time
-    names, cams, cam_of = image_table(image_dir, same_camera)
+    names, cams, cam_of = image_table(image_dir, same_camera, camera_model)
     t0 = time.time()
     kps, descs = [], []
     for name in names:

@@ -11,7 +11,8 @@ to COLMAP's output (DESIGN.md section 2).
 
 The protocol (k_mvs.cu, include/nero_mvs.h):
   * Inputs.  The model comes from objprep.read_colmap_model(tracks=True); K is the one CustomDatabase uses, so SIMPLE_RADIAL
-    distortion is ignored, as training ignores it (a limitation: strongly distorted images match worse at their borders).
+    distortion is ignored, as training ignores it (a limitation: strongly distorted images match worse at their borders;
+    undistort.py, tools/undistort_images.py, turns such a model into a pinhole project first).
     Views are taken in name order.  Pixel (x, y) is the image point (x + 1/2, y + 1/2).
   * Grey images.  From uint8 RGB, g = sum(299 R + 587 G + 114 B) / (255000 s^2) over each s x s block, the sum in integers
     and one fp32 division, s = ceil(max(w, h) / max_size); the image is (h // s) x (w // s) and K is scaled by 1 / s in x

@@ -90,64 +90,9 @@ def _read(f, fmt):
     return struct.unpack(fmt, b)
 
 
-def _read_bin(path, tracks=None):
-    cameras, images, pts = {}, {}, []
-    with open(os.path.join(path, 'cameras.bin'), 'rb') as f:
-        for _ in range(_read(f, '<Q')[0]):
-            cid, mid, w, h = _read(f, '<iiQQ')
-            if mid not in CAMERA_MODELS:
-                raise ValueError(f'{path}: unknown camera model id {mid}')
-            name, npar = CAMERA_MODELS[mid]
-            cameras[cid] = (name, w, h, _read(f, f'<{npar}d'))
-    with open(os.path.join(path, 'images.bin'), 'rb') as f:
-        for _ in range(_read(f, '<Q')[0]):
-            iid, qw, qx, qy, qz, tx, ty, tz, cid = _read(f, '<i4d3di')
-            name = bytearray()
-            while True:
-                c = f.read(1)
-                if c in (b'\x00', b''):
-                    break
-                name += c
-            f.seek(24 * _read(f, '<Q')[0], 1)                     # POINTS2D[] as (x, y double, point3D_id int64)
-            images[iid] = (name.decode('utf-8'), (qw, qx, qy, qz), (tx, ty, tz), cid)
-    with open(os.path.join(path, 'points3D.bin'), 'rb') as f:
-        for _ in range(_read(f, '<Q')[0]):
-            rec = _read(f, '<Q3d3BdQ')
-            pts.append(rec[1:4])
-            if tracks is None:
-                f.seek(8 * rec[-1], 1)                             # TRACK[] as (image_id, point2D_idx int32)
-            else:
-                tracks.append(np.asarray(_read(f, f'<{2 * rec[-1]}i')[0::2], np.int64))
-    return cameras, images, pts
-
-
 def _data_lines(path):
     with open(path) as f:
         return [ln.rstrip('\r\n') for ln in f if not ln.startswith('#')]
-
-
-def _read_txt(path, tracks=None):
-    cameras, images, pts = {}, {}, []
-    for ln in _data_lines(os.path.join(path, 'cameras.txt')):
-        e = ln.split()
-        if e:
-            cameras[int(e[0])] = (e[1], int(e[2]), int(e[3]), tuple(float(v) for v in e[4:]))
-    lines = _data_lines(os.path.join(path, 'images.txt'))
-    i = 0
-    while i < len(lines):
-        e = lines[i].split()
-        if not e:
-            i += 1
-            continue
-        images[int(e[0])] = (' '.join(e[9:]), tuple(float(v) for v in e[1:5]), tuple(float(v) for v in e[5:8]), int(e[8]))
-        i += 2                                                     # the POINTS2D line follows, possibly empty
-    for ln in _data_lines(os.path.join(path, 'points3D.txt')):
-        e = ln.split()
-        if e:
-            pts.append(tuple(float(v) for v in e[1:4]))
-            if tracks is not None:                                 # TRACK[] as (IMAGE_ID, POINT2D_IDX) after ERROR
-                tracks.append(np.asarray([int(v) for v in e[8::2]], np.int64))
-    return cameras, images, pts
 
 
 def read_colmap_model(path, tracks=False):
@@ -158,22 +103,77 @@ def read_colmap_model(path, tracks=False):
     CustomDatabase._parse_colmap builds them; points = the sparse points float64 [P,3] in file order; tracks = one int64
     array per point of the image ids of its track, in file order.  An image whose camera model is not SIMPLE_RADIAL
     (distortion ignored), SIMPLE_PINHOLE or PINHOLE raises NotImplementedError."""
-    trk = [] if tracks else None
-    if all(os.path.isfile(os.path.join(path, f'{n}.bin')) for n in ('cameras', 'images', 'points3D')):
-        cameras, images, pts = _read_bin(path, trk)
-    elif all(os.path.isfile(os.path.join(path, f'{n}.txt')) for n in ('cameras', 'images', 'points3D')):
-        cameras, images, pts = _read_txt(path, trk)
-    else:
-        raise FileNotFoundError(f'{path}: no COLMAP model (cameras, images and points3D as .bin or .txt)')
+    cameras, images, points = read_colmap_records(path)
     views = {}
-    for iid, (name, q, t, cid) in images.items():
+    for iid, (q, t, cid, name, _, _) in images.items():
         if cid not in cameras:
             raise ValueError(f'{path}: image {iid} uses camera {cid}, which the model does not define')
         pose = np.concatenate([qvec2rotmat(q), np.asarray(t, np.float64)[:, None]], 1).astype(np.float32)
         views[iid] = (name, pose, _intrinsics(cameras[cid][0], cameras[cid][3]))
+    pts = np.asarray([p[0] for p in points.values()], np.float64).reshape(-1, 3)
     if tracks:
-        return views, np.asarray(pts, np.float64).reshape(-1, 3), trk
-    return views, np.asarray(pts, np.float64).reshape(-1, 3)
+        return views, pts, [p[3] for p in points.values()]
+    return views, pts
+
+
+def read_colmap_records(path):
+    """Every record of the COLMAP model in `path` (.bin, else .txt), in the form write_colmap_model takes, in file order:
+    (cameras, images, points).  Camera parameters are kept whatever the model."""
+    cameras, images, points = {}, {}, {}
+    if all(os.path.isfile(os.path.join(path, f'{n}.bin')) for n in ('cameras', 'images', 'points3D')):
+        with open(os.path.join(path, 'cameras.bin'), 'rb') as f:
+            for _ in range(_read(f, '<Q')[0]):
+                cid, mid, w, h = _read(f, '<iiQQ')
+                if mid not in CAMERA_MODELS:
+                    raise ValueError(f'{path}: unknown camera model id {mid}')
+                name, npar = CAMERA_MODELS[mid]
+                cameras[cid] = (name, w, h, list(_read(f, f'<{npar}d')))
+        rec = np.dtype([('x', '<f8'), ('y', '<f8'), ('id', '<i8')])
+        with open(os.path.join(path, 'images.bin'), 'rb') as f:
+            for _ in range(_read(f, '<Q')[0]):
+                iid, qw, qx, qy, qz, tx, ty, tz, cid = _read(f, '<i4d3di')
+                name = bytearray()
+                while True:
+                    c = f.read(1)
+                    if c in (b'\x00', b''):
+                        break
+                    name += c
+                n = _read(f, '<Q')[0]
+                r = np.frombuffer(f.read(24 * n), rec)
+                if r.shape[0] != n:
+                    raise ValueError(f'{f.name}: truncated COLMAP file')
+                images[iid] = ((qw, qx, qy, qz), (tx, ty, tz), cid, name.decode('utf-8'), np.stack([r['x'], r['y']], 1),
+                               r['id'].astype(np.int64))
+        with open(os.path.join(path, 'points3D.bin'), 'rb') as f:
+            for _ in range(_read(f, '<Q')[0]):
+                pid, x, y, z, r_, g_, b_, err, n = _read(f, '<Q3d3BdQ')
+                tr = np.asarray(_read(f, f'<{2 * n}i'), np.int64)
+                points[pid] = ((x, y, z), [r_, g_, b_], err, tr[0::2], tr[1::2])
+        return cameras, images, points
+    if not all(os.path.isfile(os.path.join(path, f'{n}.txt')) for n in ('cameras', 'images', 'points3D')):
+        raise FileNotFoundError(f'{path}: no COLMAP model (cameras, images and points3D as .bin or .txt)')
+    for ln in _data_lines(os.path.join(path, 'cameras.txt')):
+        e = ln.split()
+        if e:
+            cameras[int(e[0])] = (e[1], int(e[2]), int(e[3]), [float(v) for v in e[4:]])
+    lines = _data_lines(os.path.join(path, 'images.txt'))
+    i = 0
+    while i < len(lines):
+        e = lines[i].split()
+        if not e:
+            i += 1
+            continue
+        p = (lines[i + 1].split() if i + 1 < len(lines) else [])
+        xys = np.asarray([float(v) for k, v in enumerate(p) if k % 3 != 2], np.float64).reshape(-1, 2)
+        images[int(e[0])] = (tuple(float(v) for v in e[1:5]), tuple(float(v) for v in e[5:8]), int(e[8]), ' '.join(e[9:]), xys,
+                             np.asarray([int(v) for v in p[2::3]], np.int64))
+        i += 2
+    for ln in _data_lines(os.path.join(path, 'points3D.txt')):
+        e = ln.split()
+        if e:
+            points[int(e[0])] = (tuple(float(v) for v in e[1:4]), [int(v) for v in e[4:7]], float(e[7]),
+                                 np.asarray([int(v) for v in e[8::2]], np.int64), np.asarray([int(v) for v in e[9::2]], np.int64))
+    return cameras, images, points
 
 
 def write_colmap_model(path, cameras, images, points):

@@ -118,7 +118,8 @@ def check_database(db):
     if bad:
         name = objprep.CAMERA_MODELS.get(db['cameras'][bad[0]][0], ('unknown',))[0]
         raise ValueError(f'camera {bad[0]} is {name}: the mapper reconstructs SIMPLE_PINHOLE cameras only (the model '
-                         'match_features.py writes); distortion models are out of its scope')
+                         'match_features.py writes); distortion models are out of its scope (a SIMPLE_RADIAL model '
+                         'from COLMAP\'s mapper is undistorted by tools/undistort_images.py)')
     if not db['pairs']:
         raise ValueError('the database has no verified image pair (two_view_geometries with inlier matches)')
 
