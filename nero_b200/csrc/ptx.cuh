@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for the sm_90a features the kernels use: mbarrier, bulk async copy (UBLKCP), the warpgroup
-// MMA (wgmma) fences and the shared-memory matrix descriptors.
+// Thin inline-PTX wrappers for the sm_90a features the kernels use: mbarrier, bulk async copy (UBLKCP) and tensor copy
+// (TMA), the warpgroup MMA (wgmma) fences and the shared-memory matrix descriptors.
 // Every spin-wait is BOUNDED: a wait that does not complete traps (kernel error) instead of hanging the GPU.
 #pragma once
 #include <cstdint>
@@ -55,6 +55,18 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if (++spins > (1u << 24)) __trap();
   }
 }
+// The same bounded wait for code that keeps wgmma groups in flight across it: a trap there makes ptxas retire every
+// wgmma before the wait (C7517, "warpgroup.wait is injected").  A wait that does not complete sets `timed_out` and
+// returns instead; the caller traps once its MMAs have drained.
+__device__ __forceinline__ void mbar_wait_flag(uint64_t* bar, uint32_t parity, bool& timed_out) {
+  uint32_t spins = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    if (++spins > (1u << 24)) {
+      timed_out = true;
+      return;
+    }
+  }
+}
 
 // make generic-proxy smem writes visible to the async proxy (wgmma / bulk copies read smem through it)
 __device__ __forceinline__ void fence_proxy_async_smem() {
@@ -87,6 +99,16 @@ __device__ __forceinline__ void bulk_copy_g2s(void* smem_dst, const void* gmem_s
       "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
           smem_u32(smem_dst)),
       "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)), "l"(l2_policy)
+      : "memory");
+}
+
+// 2-D tensor copy (TMA) of the box at coordinates (c0 = innermost, c1) of `tmap` (a __grid_constant__ kernel parameter);
+// elements outside the tensor arrive as zeros and count towards the transaction bytes
+__device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* tmap, int c0, int c1, uint64_t* bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
+          smem_u32(smem_dst)),
+      "l"(tmap), "r"(c0), "r"(c1), "r"(smem_u32(bar))
       : "memory");
 }
 

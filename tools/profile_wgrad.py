@@ -1,13 +1,15 @@
 """Per-launch profile of the weight-gradient pass of one training step (run on the GPU box).
 
-    python tools/profile_wgrad.py [--workload bell|bear] [--out DIR]      # NERO_LIB=... selects another build
+    python tools/profile_wgrad.py [--workload bell|bear] [--out DIR] [--table]     # NERO_LIB=... selects another build
 
 Warms up three resident steps of the bench workload, then records one more under torch.profiler (CUDA activities).  Every
 `gemm_wgrad_kernel<NW>` launch is matched, in issue order, to the `nero_wgrad` call that made it, which gives its rows
 (the device count, read after the step), NW, number of pairs and output rows.  Algorithmic bytes of a launch = each
 operand read once (dY columns [0, n_valid), X columns [k0, k0 + NW) clipped to k_valid, per pair) + the slice windows
 written once (P x rows x NW fp32 + the bias sums).  Also reported: `nero_wgrad_finish_batch`, the accumulator memsets
-(torch fill / zero kernels) and the step total, with the GPU name and power limit of the run.  Prints one JSON line.
+(torch fill / zero kernels) and the step total, with the GPU name and power limit of the run.  Prints one JSON line;
+`--table` also prints one line per kernel (launches, time, algorithmic GB, TB/s and share of the data-sheet HBM peak),
+the finish on a line of its own.
 """
 import argparse
 import json
@@ -41,6 +43,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--workload', default='bell', choices=['bell', 'bear'])
     ap.add_argument('--out', default=None, help='also write the JSON and the kernel table here')
+    ap.add_argument('--table', action='store_true', help='also print a per-kernel table (time, bytes, TB/s, share of peak)')
     args = ap.parse_args()
     dev = torch.device('cuda')
     wl = bench.Workload(args.workload == 'bear', 0, 1, dev)
@@ -121,6 +124,15 @@ def main():
         t[1] += e.device_time
     res['top_kernels'] = [[k, n, round(us / 1e3, 3)] for k, (n, us) in sorted(top.items(), key=lambda kv: -kv[1][1])[:14]]
     print(json.dumps(res))
+    if args.table:
+        print(f'# {res["gpu"].get("name")} at {res["gpu"].get("power_limit")}, peak {HBM_PEAK / 1e12:.2f} TB/s (data sheet)')
+        print(f'{"kernel":28s} {"launches":>8s} {"ms":>8s} {"GB":>8s} {"TB/s":>7s} {"of peak":>8s}')
+        for k, d in sorted(by_nw.items()):
+            tbs = d['bytes'] / (d['ms'] * 1e-3) / 1e12 if d['ms'] else 0.0
+            print(f'{k:28s} {d["launches"]:8d} {d["ms"]:8.3f} {d["bytes"] / 1e9:8.2f} {tbs:7.3f} {tbs * 1e12 / HBM_PEAK:8.1%}')
+        fb = res['finish_batch']
+        print(f'{"nero_wgrad_finish_batch":28s} {fb["launches"]:8d} {fb["ms"]:8.3f}')
+        print(f'{"whole pass":28s} {"":8s} {res["wgrad_pass_ms"]:8.3f}')
     if args.out:
         os.makedirs(args.out, exist_ok=True)
         with open(os.path.join(args.out, f'wgrad_{args.workload}_{os.path.basename(res["lib"])}.json'), 'w') as f:
