@@ -20,6 +20,7 @@
 #include "hash.cuh"
 #include "union_find.cuh"
 #include "../../include/nero_sfm.h"
+#include "../../include/nero_sfm_radial.h"
 
 namespace nero {
 namespace {
@@ -133,22 +134,35 @@ __device__ __forceinline__ void rotate_left(const double w[3], const double R[9]
     for (int c = 0; c < 3; ++c) out[3 * r + c] = E[3 * r] * R[c] + E[3 * r + 1] * R[3 + c] + E[3 * r + 2] * R[6 + c];
 }
 
-// camera-frame point, its projection residual and the unit ray from the camera centre
+// camera-frame point, its projection residual and the unit ray from the camera centre.  kCam is the number of free
+// parameters of a camera: 1 (SIMPLE_PINHOLE: f) or 2 (SIMPLE_RADIAL: f, k; include/nero_sfm_radial.h).
 struct Cam {
-  double R[9], t[3], f, cx, cy;
+  double R[9], t[3], f, cx, cy, k;
 };
 
-__device__ __forceinline__ Cam load_cam(const double* pose, const int* img_cam, const double* focal, const double* pp, int i) {
+template <int kCam = 1>
+__device__ __forceinline__ Cam load_cam(const double* pose, const int* img_cam, const double* focal, const double* pp, int i,
+                                        const double* radial = nullptr) {
   Cam c;
   load_pose(pose, i, c.R, c.t);
   const int k = img_cam[i];
   c.f = focal[k];
   c.cx = pp[2 * k];
   c.cy = pp[2 * k + 1];
+  c.k = kCam == 2 ? radial[k] : 0.0;
   return c;
 }
 
-// (depth, squared reprojection error) of X seen at (x, y)
+// SIMPLE_RADIAL: normalised point (x, y) = (Y_x, Y_y) / Y_z, r2 = x^2 + y^2, d = 1 + k r2, pixel ((f x) d + cx, (f y) d + cy)
+__device__ __forceinline__ void radial_pixel(const Cam& c, double x, double y, double* r2, double* d, double* pu, double* pv) {
+  *r2 = x * x + y * y;
+  *d = 1.0 + c.k * *r2;
+  *pu = (c.f * x) * *d + c.cx;
+  *pv = (c.f * y) * *d + c.cy;
+}
+
+// (depth, squared reprojection error) of X seen at (x, y), in the (distorted) image
+template <int kCam = 1>
 __device__ __forceinline__ double reproj2(const Cam& c, const double X[3], double x, double y, double* depth) {
   double Y[3];
   mat3_vec(c.R, X, Y);
@@ -156,7 +170,17 @@ __device__ __forceinline__ double reproj2(const Cam& c, const double X[3], doubl
   Y[1] += c.t[1];
   Y[2] += c.t[2];
   *depth = Y[2];
-  const double ex = c.f * Y[0] / Y[2] + c.cx - x, ey = c.f * Y[1] / Y[2] + c.cy - y;
+  double ex, ey;
+  if constexpr (kCam == 1) {
+    ex = c.f * Y[0] / Y[2] + c.cx - x;
+    ey = c.f * Y[1] / Y[2] + c.cy - y;
+  } else {
+    const double iz = 1.0 / Y[2];
+    double r2, d, pu, pv;
+    radial_pixel(c, Y[0] * iz, Y[1] * iz, &r2, &d, &pu, &pv);
+    ex = pu - x;
+    ey = pv - y;
+  }
   return ex * ex + ey * ey;
 }
 
@@ -581,19 +605,21 @@ __global__ void __launch_bounds__(kBlock) triangulate_kernel(const long long* __
   stat[3 * k + 2] = largest_angle(o0, o1, obs_img, pose, img_cam, focal, pp, X);
 }
 
+template <int kCam>
 __global__ void __launch_bounds__(kBlock) filter_kernel(const long long* __restrict__ pt_off, int P, const int* __restrict__ obs_img,
                                                         const double* __restrict__ obs_xy, const double* __restrict__ pose,
                                                         const int* __restrict__ img_cam, const double* __restrict__ focal,
                                                         const double* __restrict__ pp, const double* __restrict__ Xin,
-                                                        double* __restrict__ err, double* __restrict__ angle) {
+                                                        double* __restrict__ err, double* __restrict__ angle,
+                                                        const double* __restrict__ radial) {
   const int p = blockIdx.x * kBlock + threadIdx.x;
   if (p >= P) return;
   const double X[3] = {Xin[3 * p], Xin[3 * p + 1], Xin[3 * p + 2]};
   const long long o0 = pt_off[p], o1 = pt_off[p + 1];
   for (long long o = o0; o < o1; ++o) {
-    const Cam c = load_cam(pose, img_cam, focal, pp, obs_img[o]);
+    const Cam c = load_cam<kCam>(pose, img_cam, focal, pp, obs_img[o], radial);
     double z;
-    const double e2 = reproj2(c, X, obs_xy[2 * o], obs_xy[2 * o + 1], &z);
+    const double e2 = reproj2<kCam>(c, X, obs_xy[2 * o], obs_xy[2 * o + 1], &z);
     err[2 * o] = z;
     err[2 * o + 1] = sqrt(e2);
   }
@@ -601,49 +627,98 @@ __global__ void __launch_bounds__(kBlock) filter_kernel(const long long* __restr
 }
 
 // ------------------------------------------------------------------------------------------------ bundle adjustment
+// Per observation the camera-side columns are (w, t) and the kCam camera parameters: kNc = 6 + kCam of them.  Jc is
+// [n, 2, kNc], Y [n, kNc, 3].
+template <int kCam>
+constexpr int kNc = 6 + kCam;
+
+// Residual res [2] of Y = R X + t seen at xy [2], its derivative dY [2][3] with respect to Y, and the camera-parameter
+// columns jf [2][kCam].  Pinhole: dr/dY = (f / Y_z) [[1, 0, -u], [0, 1, -v]], dr/df = (u, v).  Radial, with (x, y) the
+// normalised point: dr/d(x, y) = f [[d + 2k x^2, 2k x y], [2k x y, d + 2k y^2]], d(x, y)/dY = (1 / Y_z) [[1, 0, -x],
+// [0, 1, -y]], dr/df = (x d, y d), dr/dk = (f x r2, f y r2).
+template <int kCam>
+__device__ __forceinline__ void project_jacobian(const Cam& c, const double Y[3], const double* __restrict__ xy, double* __restrict__ res,
+                                                 double dY[2][3], double jf[2][kCam]) {
+  const double iz = 1.0 / Y[2], u = Y[0] * iz, v = Y[1] * iz;
+  if constexpr (kCam == 1) {
+    const double fz = c.f * iz;
+    res[0] = c.f * u + c.cx - xy[0];
+    res[1] = c.f * v + c.cy - xy[1];
+    dY[0][0] = fz;
+    dY[0][1] = 0.0;
+    dY[0][2] = -fz * u;
+    dY[1][0] = 0.0;
+    dY[1][1] = fz;
+    dY[1][2] = -fz * v;
+    jf[0][0] = u;
+    jf[1][0] = v;
+  } else {
+    double r2, d, pu, pv;
+    radial_pixel(c, u, v, &r2, &d, &pu, &pv);
+    res[0] = pu - xy[0];
+    res[1] = pv - xy[1];
+    const double a = c.f * (d + 2.0 * c.k * u * u), b = c.f * (2.0 * c.k * u * v), e = c.f * (d + 2.0 * c.k * v * v);
+    dY[0][0] = a * iz;
+    dY[0][1] = b * iz;
+    dY[0][2] = -(a * u + b * v) * iz;
+    dY[1][0] = b * iz;
+    dY[1][1] = e * iz;
+    dY[1][2] = -(b * u + e * v) * iz;
+    jf[0][0] = u * d;
+    jf[1][0] = v * d;
+    jf[0][1] = c.f * u * r2;
+    jf[1][1] = c.f * v * r2;
+  }
+}
+
+template <int kCam>
 __global__ void __launch_bounds__(kBlock) linearize_kernel(const long long* __restrict__ pt_off, int P, const int* __restrict__ obs_img,
                                                            const double* __restrict__ obs_xy, const double* __restrict__ pose,
                                                            const int* __restrict__ img_cam, const double* __restrict__ focal,
                                                            const double* __restrict__ pp, const double* __restrict__ Xin,
-                                                           double* __restrict__ res, double* __restrict__ Jc, double* __restrict__ Jp) {
+                                                           double* __restrict__ res, double* __restrict__ Jc, double* __restrict__ Jp,
+                                                           const double* __restrict__ radial) {
+  constexpr int NC = kNc<kCam>;
   const int p = blockIdx.x * kBlock + threadIdx.x;
   if (p >= P) return;
   const double X[3] = {Xin[3 * p], Xin[3 * p + 1], Xin[3 * p + 2]};
   for (long long o = pt_off[p]; o < pt_off[p + 1]; ++o) {
-    const Cam c = load_cam(pose, img_cam, focal, pp, obs_img[o]);
+    const Cam c = load_cam<kCam>(pose, img_cam, focal, pp, obs_img[o], radial);
     double RX[3];
     mat3_vec(c.R, X, RX);
     const double Y[3] = {RX[0] + c.t[0], RX[1] + c.t[1], RX[2] + c.t[2]};
-    const double iz = 1.0 / Y[2], u = Y[0] * iz, v = Y[1] * iz, fz = c.f * iz;
-    res[2 * o] = c.f * u + c.cx - obs_xy[2 * o];
-    res[2 * o + 1] = c.f * v + c.cy - obs_xy[2 * o + 1];
-    // dr/dY = fz [[1, 0, -u], [0, 1, -v]]; dY/dw = -[RX]x; dY/dt = I; dY/dX = R
-    const double dY[2][3] = {{fz, 0.0, -fz * u}, {0.0, fz, -fz * v}};
+    double dY[2][3], jf[2][kCam];
+    project_jacobian<kCam>(c, Y, obs_xy + 2 * o, res + 2 * o, dY, jf);
+    // dY/dw = -[RX]x; dY/dt = I; dY/dX = R
     const double H[9] = {0.0, RX[2], -RX[1], -RX[2], 0.0, RX[0], RX[1], -RX[0], 0.0};   // -[RX]x
-    double* jc = Jc + 14 * o;
+    double* jc = Jc + 2 * NC * o;
     double* jp = Jp + 6 * o;
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
 #pragma unroll
       for (int q = 0; q < 3; ++q) {
-        jc[7 * r + q] = dY[r][0] * H[q] + dY[r][1] * H[3 + q] + dY[r][2] * H[6 + q];
-        jc[7 * r + 3 + q] = dY[r][q];
+        jc[NC * r + q] = dY[r][0] * H[q] + dY[r][1] * H[3 + q] + dY[r][2] * H[6 + q];
+        jc[NC * r + 3 + q] = dY[r][q];
         jp[3 * r + q] = dY[r][0] * c.R[q] + dY[r][1] * c.R[3 + q] + dY[r][2] * c.R[6 + q];
       }
-      jc[7 * r + 6] = r == 0 ? u : v;
+#pragma unroll
+      for (int q = 0; q < kCam; ++q) jc[NC * r + 6 + q] = jf[r][q];
     }
   }
 }
 
 // W_o [a][k] = (Jc_o^T Jp_o) [a][k]
+template <int NC>
 __device__ __forceinline__ double w_entry(const double* jc, const double* jp, int a, int k) {
-  return jc[a] * jp[k] + jc[7 + a] * jp[3 + k];
+  return jc[a] * jp[k] + jc[NC + a] * jp[3 + k];
 }
 
+template <int kCam>
 __global__ void __launch_bounds__(kBlock) points_kernel(const long long* __restrict__ pt_off, int P, const double* __restrict__ res,
                                                         const double* __restrict__ Jc, const double* __restrict__ Jp, double lambda,
                                                         int fix_points, double* __restrict__ Vinv, double* __restrict__ gp,
                                                         double* __restrict__ Y) {
+  constexpr int NC = kNc<kCam>;
   const int p = blockIdx.x * kBlock + threadIdx.x;
   if (p >= P) return;
   const long long o0 = pt_off[p], o1 = pt_off[p + 1];
@@ -670,25 +745,28 @@ __global__ void __launch_bounds__(kBlock) points_kernel(const long long* __restr
 #pragma unroll
   for (int e = 0; e < 3; ++e) gp[3 * p + e] = g[e];
   for (long long o = o0; o < o1; ++o) {
-    const double* jc = Jc + 14 * o;
+    const double* jc = Jc + 2 * NC * o;
     const double* jp = Jp + 6 * o;
 #pragma unroll
-    for (int a = 0; a < 7; ++a) {
-      const double w0 = w_entry(jc, jp, a, 0), w1 = w_entry(jc, jp, a, 1), w2 = w_entry(jc, jp, a, 2);
+    for (int a = 0; a < NC; ++a) {
+      const double w0 = w_entry<NC>(jc, jp, a, 0), w1 = w_entry<NC>(jc, jp, a, 1), w2 = w_entry<NC>(jc, jp, a, 2);
 #pragma unroll
-      for (int k = 0; k < 3; ++k) Y[21 * o + 3 * a + k] = w0 * Vi[k] + w1 * Vi[3 + k] + w2 * Vi[6 + k];
+      for (int k = 0; k < 3; ++k) Y[3 * NC * o + 3 * a + k] = w0 * Vi[k] + w1 * Vi[3 + k] + w2 * Vi[6 + k];
     }
   }
 }
 
+// block b < nimg: image b's 6 columns at 6 b; block nimg + c: camera c's kCam columns at 6 nimg + kCam c, local columns
+// 6 .. 5 + kCam of an observation
+template <int kCam>
 __device__ __forceinline__ void block_geom(int blk, int nimg, int* col0, int* width, int* local0) {
   if (blk < nimg) {
     *col0 = 6 * blk;
     *width = 6;
     *local0 = 0;
   } else {
-    *col0 = 6 * nimg + (blk - nimg);
-    *width = 1;
+    *col0 = 6 * nimg + kCam * (blk - nimg);
+    *width = kCam;
     *local0 = 6;
   }
 }
@@ -698,48 +776,52 @@ constexpr int kReduceThreads = 64;
 // Stage 1 of the reduced system: one block per chunk (at most NERO_SFM_CHUNK consecutive entries of one segment), one
 // thread per entry of the (row block, column block) pair, summed in entry order into partial [chunk, 36] (slot 6 r + c).
 // The damping is applied per chunk: (1 + lambda) u + s sums to (1 + lambda) U + S over the chunks.
+template <int kCam>
 __global__ void __launch_bounds__(kReduceThreads) reduce_chunk_kernel(const int* __restrict__ ent, const long long* __restrict__ chunk,
                                                                       const int* __restrict__ chunk_key, int nimg, const double* __restrict__ Jc,
                                                                       const double* __restrict__ Jp, const double* __restrict__ Y, double lambda,
                                                                       double* __restrict__ partial) {
+  constexpr int NC = kNc<kCam>;
   const int k = blockIdx.x;
   int r0, rw, rl, c0, cw, cl;
-  block_geom(chunk_key[2 * k], nimg, &r0, &rw, &rl);
-  block_geom(chunk_key[2 * k + 1], nimg, &c0, &cw, &cl);
+  block_geom<kCam>(chunk_key[2 * k], nimg, &r0, &rw, &rl);
+  block_geom<kCam>(chunk_key[2 * k + 1], nimg, &c0, &cw, &cl);
   const int r = threadIdx.x / 6, c = threadIdx.x % 6;
   if (r >= rw || c >= cw) return;
   const int lr = rl + r, lc = cl + c;
   double u = 0.0, sc = 0.0;
   for (long long e = chunk[2 * k]; e < chunk[2 * k + 1]; ++e) {
     const int o = ent[2 * e], o2 = ent[2 * e + 1];
-    const double* jc2 = Jc + 14 * (long long)o2;
+    const double* jc2 = Jc + 2 * NC * (long long)o2;
     const double* jp2 = Jp + 6 * (long long)o2;
-    if (o == o2) u += jc2[lr] * jc2[lc] + jc2[7 + lr] * jc2[7 + lc];
-    const double* y = Y + 21 * (long long)o + 3 * lr;
-    sc -= y[0] * w_entry(jc2, jp2, lc, 0) + y[1] * w_entry(jc2, jp2, lc, 1) + y[2] * w_entry(jc2, jp2, lc, 2);
+    if (o == o2) u += jc2[lr] * jc2[lc] + jc2[NC + lr] * jc2[NC + lc];
+    const double* y = Y + 3 * NC * (long long)o + 3 * lr;
+    sc -= y[0] * w_entry<NC>(jc2, jp2, lc, 0) + y[1] * w_entry<NC>(jc2, jp2, lc, 1) + y[2] * w_entry<NC>(jc2, jp2, lc, 2);
   }
   partial[36 * (long long)k + 6 * r + c] = r0 + r == c0 + c ? u + lambda * u + sc : u + sc;
 }
 
 // Stage 1 of the right-hand side: one block per chunk of one block's observation list, partial [chunk, 6] (slot r)
+template <int kCam>
 __global__ void __launch_bounds__(kReduceThreads) rhs_chunk_kernel(const int* __restrict__ obs_seg, const long long* __restrict__ chunk,
                                                                    const int* __restrict__ chunk_blk, const int* __restrict__ obs_pt, int nimg,
                                                                    const double* __restrict__ Jc, const double* __restrict__ res,
                                                                    const double* __restrict__ Y, const double* __restrict__ gp,
                                                                    double* __restrict__ partial) {
+  constexpr int NC = kNc<kCam>;
   const int k = blockIdx.x;
   int r0, rw, rl;
-  block_geom(chunk_blk[k], nimg, &r0, &rw, &rl);
+  block_geom<kCam>(chunk_blk[k], nimg, &r0, &rw, &rl);
   const int r = threadIdx.x;
   if (r >= rw) return;
   const int lr = rl + r;
   double acc = 0.0;
   for (long long e = chunk[2 * k]; e < chunk[2 * k + 1]; ++e) {
     const int o = obs_seg[2 * e];
-    const double* jc = Jc + 14 * (long long)o;
-    const double* y = Y + 21 * (long long)o + 3 * lr;
+    const double* jc = Jc + 2 * NC * (long long)o;
+    const double* y = Y + 3 * NC * (long long)o + 3 * lr;
     const double* g = gp + 3 * (long long)obs_pt[o];
-    acc += jc[lr] * res[2 * (long long)o] + jc[7 + lr] * res[2 * (long long)o + 1] - (y[0] * g[0] + y[1] * g[1] + y[2] * g[2]);
+    acc += jc[lr] * res[2 * (long long)o] + jc[NC + lr] * res[2 * (long long)o + 1] - (y[0] * g[0] + y[1] * g[1] + y[2] * g[2]);
   }
   partial[6 * (long long)k + r] = acc;
 }
@@ -747,7 +829,7 @@ __global__ void __launch_bounds__(kReduceThreads) rhs_chunk_kernel(const int* __
 // Stage 2: one block per segment adds its chunks' partials in a fixed shape: thread t sums chunks t, t + 64, ... in
 // order, then a fixed tree over the 64 threads.  kSlots = 36 writes S (fixed parameters: the identity), kSlots = 6 writes
 // b = -sum (fixed parameters: 0).
-template <int kSlots>
+template <int kSlots, int kCam>
 __global__ void __launch_bounds__(kReduceThreads) segment_sum_kernel(const long long* __restrict__ seg_chunk, const int* __restrict__ seg_key,
                                                                      int nimg, int ncol, const double* __restrict__ partial,
                                                                      const unsigned char* __restrict__ fixed, double* __restrict__ out) {
@@ -755,10 +837,10 @@ __global__ void __launch_bounds__(kReduceThreads) segment_sum_kernel(const long 
   const int s = blockIdx.x, t = threadIdx.x;
   int r0, rw, rl, c0 = 0, cw = 1, cl = 0;
   if (kSlots == 36) {
-    block_geom(seg_key[2 * s], nimg, &r0, &rw, &rl);
-    block_geom(seg_key[2 * s + 1], nimg, &c0, &cw, &cl);
+    block_geom<kCam>(seg_key[2 * s], nimg, &r0, &rw, &rl);
+    block_geom<kCam>(seg_key[2 * s + 1], nimg, &c0, &cw, &cl);
   } else {
-    block_geom(seg_key[s], nimg, &r0, &rw, &rl);
+    block_geom<kCam>(seg_key[s], nimg, &r0, &rw, &rl);
   }
   double acc[kSlots];
 #pragma unroll
@@ -792,30 +874,34 @@ __global__ void __launch_bounds__(kReduceThreads) segment_sum_kernel(const long 
   }
 }
 
+template <int kCam>
 __global__ void __launch_bounds__(kBlock) backsub_kernel(const long long* __restrict__ pt_off, int P, const int* __restrict__ obs_img,
                                                          const int* __restrict__ img_cam, int nimg, int ncam, const double* __restrict__ Jc,
                                                          const double* __restrict__ Jp, const double* __restrict__ Vinv,
                                                          const double* __restrict__ gp, const double* __restrict__ dc,
                                                          const double* __restrict__ pose, const double* __restrict__ focal,
                                                          const double* __restrict__ Xin, double* __restrict__ pose_new,
-                                                         double* __restrict__ focal_new, double* __restrict__ X_new) {
+                                                         double* __restrict__ focal_new, double* __restrict__ X_new,
+                                                         const double* __restrict__ radial, double* __restrict__ radial_new) {
+  constexpr int NC = kNc<kCam>;
   const long long idx = (long long)blockIdx.x * kBlock + threadIdx.x;
   if (idx < P) {
     const int p = (int)idx;
     double acc[3] = {gp[3 * p], gp[3 * p + 1], gp[3 * p + 2]};
     for (long long o = pt_off[p]; o < pt_off[p + 1]; ++o) {
       const int i = obs_img[o];
-      double d7[7];
+      double dn[NC];
 #pragma unroll
-      for (int a = 0; a < 6; ++a) d7[a] = dc[6 * i + a];
-      d7[6] = dc[6 * nimg + img_cam[i]];
-      const double* jc = Jc + 14 * o;
+      for (int a = 0; a < 6; ++a) dn[a] = dc[6 * i + a];
+#pragma unroll
+      for (int a = 0; a < kCam; ++a) dn[6 + a] = dc[6 * nimg + kCam * img_cam[i] + a];
+      const double* jc = Jc + 2 * NC * o;
       const double* jp = Jp + 6 * o;
 #pragma unroll
       for (int k = 0; k < 3; ++k) {
         double s = 0.0;
 #pragma unroll
-        for (int a = 0; a < 7; ++a) s += w_entry(jc, jp, a, k) * d7[a];
+        for (int a = 0; a < NC; ++a) s += w_entry<NC>(jc, jp, a, k) * dn[a];
         acc[k] += s;
       }
     }
@@ -836,24 +922,26 @@ __global__ void __launch_bounds__(kBlock) backsub_kernel(const long long* __rest
     for (int e = 0; e < 3; ++e) pose_new[12 * i + 9 + e] = t[e] + dc[6 * i + 3 + e];
   } else if (idx < (long long)P + nimg + ncam) {
     const int c = (int)(idx - P - nimg);
-    focal_new[c] = focal[c] + dc[6 * nimg + c];
+    focal_new[c] = focal[c] + dc[6 * nimg + kCam * c];
+    if constexpr (kCam == 2) radial_new[c] = radial[c] + dc[6 * nimg + 2 * c + 1];
   }
 }
 
+template <int kCam>
 __global__ void __launch_bounds__(kBlock) cost_kernel(const long long* __restrict__ pt_off, int P, const int* __restrict__ obs_img,
                                                       const double* __restrict__ obs_xy, const double* __restrict__ pose,
                                                       const int* __restrict__ img_cam, const double* __restrict__ focal,
                                                       const double* __restrict__ pp, const double* __restrict__ Xin,
-                                                      double* __restrict__ partial) {
+                                                      double* __restrict__ partial, const double* __restrict__ radial) {
   __shared__ double s_v[kBlock];
   const int p = blockIdx.x * kBlock + threadIdx.x;
   double acc = 0.0;
   if (p < P) {
     const double X[3] = {Xin[3 * p], Xin[3 * p + 1], Xin[3 * p + 2]};
     for (long long o = pt_off[p]; o < pt_off[p + 1]; ++o) {
-      const Cam c = load_cam(pose, img_cam, focal, pp, obs_img[o]);
+      const Cam c = load_cam<kCam>(pose, img_cam, focal, pp, obs_img[o], radial);
       double z;
-      acc += reproj2(c, X, obs_xy[2 * o], obs_xy[2 * o + 1], &z);
+      acc += reproj2<kCam>(c, X, obs_xy[2 * o], obs_xy[2 * o + 1], &z);
     }
   }
   s_v[threadIdx.x] = acc;
@@ -869,6 +957,33 @@ __global__ void cost_sum_kernel(const double* __restrict__ partial, int nblk, do
   double s = 0.0;
   for (int k = 0; k < nblk; ++k) s += partial[k];
   cost[0] = s;
+}
+
+// the reduced system of either camera model (kCam parameters per camera), checked and launched
+template <int kCam>
+int reduce(const int* ent, const long long* chunk, const int* chunk_key, int nchunk, const long long* seg_chunk, const int* seg_key,
+           int nseg, const int* obs_seg, const long long* rchunk, const int* rchunk_blk, int nrchunk, const long long* rseg_chunk,
+           const int* rseg_blk, int nrseg, const int* obs_pt, const int* img_cam, int nimg, int ncam, const double* Jc,
+           const double* Jp, const double* res, const double* Y, const double* gp, double lambda, const unsigned char* fixed,
+           double* partial, double* rpartial, double* S, double* b, void* stream) {
+  if (nchunk < 0 || nseg < 0 || nrchunk < 0 || nrseg < 0 || nimg < 1 || nimg > NERO_SFM_MAX_IMAGES || ncam < 1 || ncam > nimg ||
+      !(lambda >= 0.0) || !fixed || !S || !b || (nchunk > 0) != (nseg > 0) || (nrchunk > 0) != (nrseg > 0) ||
+      (nchunk > 0 && (!ent || !chunk || !chunk_key || !seg_chunk || !seg_key || !Jc || !Jp || !Y || !partial)) ||
+      (nrchunk > 0 && (!obs_seg || !rchunk || !rchunk_blk || !rseg_chunk || !rseg_blk || !obs_pt || !img_cam || !Jc || !res || !Y || !gp ||
+                       !rpartial)))
+    return NERO_ERR_ARG;
+  const cudaStream_t s = (cudaStream_t)stream;
+  const int ncol = 6 * nimg + kCam * ncam;
+  if (nchunk > 0) {
+    reduce_chunk_kernel<kCam><<<nchunk, kReduceThreads, 0, s>>>(ent, chunk, chunk_key, nimg, Jc, Jp, Y, lambda, partial);
+    segment_sum_kernel<36, kCam><<<nseg, kReduceThreads, 0, s>>>(seg_chunk, seg_key, nimg, ncol, partial, fixed, S);
+  }
+  if (nrchunk > 0) {
+    rhs_chunk_kernel<kCam><<<nrchunk, kReduceThreads, 0, s>>>(obs_seg, rchunk, rchunk_blk, obs_pt, nimg, Jc, res, Y, gp, rpartial);
+    segment_sum_kernel<6, kCam><<<nrseg, kReduceThreads, 0, s>>>(rseg_chunk, rseg_blk, nimg, ncol, rpartial, fixed, b);
+  }
+  NERO_LAUNCH_CHECK();
+  return NERO_OK;
 }
 
 }  // namespace
@@ -917,7 +1032,7 @@ int nero_sfm_filter(const long long* pt_off, int P, const int* obs_img, const do
                     const double* focal, const double* pp, const double* X, double* err, double* angle, void* stream) {
   if (P < 0 || (P > 0 && (!pt_off || !obs_img || !obs_xy || !pose || !img_cam || !focal || !pp || !X || !err || !angle))) return NERO_ERR_ARG;
   if (P == 0) return NERO_OK;
-  filter_kernel<<<blocks(P), kBlock, 0, (cudaStream_t)stream>>>(pt_off, P, obs_img, obs_xy, pose, img_cam, focal, pp, X, err, angle);
+  filter_kernel<1><<<blocks(P), kBlock, 0, (cudaStream_t)stream>>>(pt_off, P, obs_img, obs_xy, pose, img_cam, focal, pp, X, err, angle, nullptr);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
@@ -928,7 +1043,8 @@ int nero_sfm_ba_linearize(const long long* pt_off, int P, const int* obs_img, co
   if (P < 0 || (P > 0 && (!pt_off || !obs_img || !obs_xy || !pose || !img_cam || !focal || !pp || !X || !res || !Jc || !Jp)))
     return NERO_ERR_ARG;
   if (P == 0) return NERO_OK;
-  linearize_kernel<<<blocks(P), kBlock, 0, (cudaStream_t)stream>>>(pt_off, P, obs_img, obs_xy, pose, img_cam, focal, pp, X, res, Jc, Jp);
+  linearize_kernel<1><<<blocks(P), kBlock, 0, (cudaStream_t)stream>>>(pt_off, P, obs_img, obs_xy, pose, img_cam, focal, pp, X, res, Jc, Jp,
+                                                                      nullptr);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
@@ -937,7 +1053,7 @@ int nero_sfm_ba_points(const long long* pt_off, int P, const double* res, const 
                        double* Vinv, double* gp, double* Y, void* stream) {
   if (P < 0 || !(lambda >= 0.0) || (P > 0 && (!pt_off || !res || !Jc || !Jp || !Vinv || !gp || !Y))) return NERO_ERR_ARG;
   if (P == 0) return NERO_OK;
-  points_kernel<<<blocks(P), kBlock, 0, (cudaStream_t)stream>>>(pt_off, P, res, Jc, Jp, lambda, fix_points, Vinv, gp, Y);
+  points_kernel<1><<<blocks(P), kBlock, 0, (cudaStream_t)stream>>>(pt_off, P, res, Jc, Jp, lambda, fix_points, Vinv, gp, Y);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
@@ -947,24 +1063,8 @@ int nero_sfm_ba_reduce(const int* ent, const long long* chunk, const int* chunk_
                        const int* rseg_blk, int nrseg, const int* obs_pt, const int* img_cam, int nimg, int ncam, const double* Jc,
                        const double* Jp, const double* res, const double* Y, const double* gp, double lambda, const unsigned char* fixed,
                        double* partial, double* rpartial, double* S, double* b, void* stream) {
-  if (nchunk < 0 || nseg < 0 || nrchunk < 0 || nrseg < 0 || nimg < 1 || nimg > NERO_SFM_MAX_IMAGES || ncam < 1 || ncam > nimg ||
-      !(lambda >= 0.0) || !fixed || !S || !b || (nchunk > 0) != (nseg > 0) || (nrchunk > 0) != (nrseg > 0) ||
-      (nchunk > 0 && (!ent || !chunk || !chunk_key || !seg_chunk || !seg_key || !Jc || !Jp || !Y || !partial)) ||
-      (nrchunk > 0 && (!obs_seg || !rchunk || !rchunk_blk || !rseg_chunk || !rseg_blk || !obs_pt || !img_cam || !Jc || !res || !Y || !gp ||
-                       !rpartial)))
-    return NERO_ERR_ARG;
-  const cudaStream_t s = (cudaStream_t)stream;
-  const int ncol = 6 * nimg + ncam;
-  if (nchunk > 0) {
-    reduce_chunk_kernel<<<nchunk, kReduceThreads, 0, s>>>(ent, chunk, chunk_key, nimg, Jc, Jp, Y, lambda, partial);
-    segment_sum_kernel<36><<<nseg, kReduceThreads, 0, s>>>(seg_chunk, seg_key, nimg, ncol, partial, fixed, S);
-  }
-  if (nrchunk > 0) {
-    rhs_chunk_kernel<<<nrchunk, kReduceThreads, 0, s>>>(obs_seg, rchunk, rchunk_blk, obs_pt, nimg, Jc, res, Y, gp, rpartial);
-    segment_sum_kernel<6><<<nrseg, kReduceThreads, 0, s>>>(rseg_chunk, rseg_blk, nimg, ncol, rpartial, fixed, b);
-  }
-  NERO_LAUNCH_CHECK();
-  return NERO_OK;
+  return reduce<1>(ent, chunk, chunk_key, nchunk, seg_chunk, seg_key, nseg, obs_seg, rchunk, rchunk_blk, nrchunk, rseg_chunk, rseg_blk, nrseg,
+                   obs_pt, img_cam, nimg, ncam, Jc, Jp, res, Y, gp, lambda, fixed, partial, rpartial, S, b, stream);
 }
 
 int nero_sfm_ba_backsub(const long long* pt_off, int P, const int* obs_img, const int* img_cam, int nimg, int ncam, const double* Jc,
@@ -973,8 +1073,9 @@ int nero_sfm_ba_backsub(const long long* pt_off, int P, const int* obs_img, cons
   if (P < 0 || nimg < 1 || ncam < 1 || !dc || !pose || !focal || !pose_new || !focal_new || !img_cam ||
       (P > 0 && (!pt_off || !obs_img || !Jc || !Jp || !Vinv || !gp || !X || !X_new)))
     return NERO_ERR_ARG;
-  backsub_kernel<<<blocks((long long)P + nimg + ncam), kBlock, 0, (cudaStream_t)stream>>>(pt_off, P, obs_img, img_cam, nimg, ncam, Jc, Jp, Vinv,
-                                                                                          gp, dc, pose, focal, X, pose_new, focal_new, X_new);
+  backsub_kernel<1><<<blocks((long long)P + nimg + ncam), kBlock, 0, (cudaStream_t)stream>>>(pt_off, P, obs_img, img_cam, nimg, ncam, Jc, Jp,
+                                                                                             Vinv, gp, dc, pose, focal, X, pose_new, focal_new,
+                                                                                             X_new, nullptr, nullptr);
   NERO_LAUNCH_CHECK();
   return NERO_OK;
 }
@@ -984,7 +1085,75 @@ int nero_sfm_ba_cost(const long long* pt_off, int P, const int* obs_img, const d
   if (P < 1 || !pt_off || !obs_img || !obs_xy || !pose || !img_cam || !focal || !pp || !X || !partial || !cost) return NERO_ERR_ARG;
   const cudaStream_t s = (cudaStream_t)stream;
   const unsigned nb = blocks(P);
-  cost_kernel<<<nb, kBlock, 0, s>>>(pt_off, P, obs_img, obs_xy, pose, img_cam, focal, pp, X, partial);
+  cost_kernel<1><<<nb, kBlock, 0, s>>>(pt_off, P, obs_img, obs_xy, pose, img_cam, focal, pp, X, partial, nullptr);
+  cost_sum_kernel<<<1, 1, 0, s>>>(partial, (int)nb, cost);
+  NERO_LAUNCH_CHECK();
+  return NERO_OK;
+}
+
+int nero_sfm_radial_filter(const long long* pt_off, int P, const int* obs_img, const double* obs_xy, const double* pose, const int* img_cam,
+                           const double* focal, const double* pp, const double* radial, const double* X, double* err, double* angle,
+                           void* stream) {
+  if (P < 0 || (P > 0 && (!pt_off || !obs_img || !obs_xy || !pose || !img_cam || !focal || !pp || !radial || !X || !err || !angle)))
+    return NERO_ERR_ARG;
+  if (P == 0) return NERO_OK;
+  filter_kernel<2><<<blocks(P), kBlock, 0, (cudaStream_t)stream>>>(pt_off, P, obs_img, obs_xy, pose, img_cam, focal, pp, X, err, angle, radial);
+  NERO_LAUNCH_CHECK();
+  return NERO_OK;
+}
+
+int nero_sfm_radial_ba_linearize(const long long* pt_off, int P, const int* obs_img, const double* obs_xy, const double* pose,
+                                 const int* img_cam, const double* focal, const double* pp, const double* radial, const double* X,
+                                 double* res, double* Jc, double* Jp, void* stream) {
+  if (P < 0 || (P > 0 && (!pt_off || !obs_img || !obs_xy || !pose || !img_cam || !focal || !pp || !radial || !X || !res || !Jc || !Jp)))
+    return NERO_ERR_ARG;
+  if (P == 0) return NERO_OK;
+  linearize_kernel<2><<<blocks(P), kBlock, 0, (cudaStream_t)stream>>>(pt_off, P, obs_img, obs_xy, pose, img_cam, focal, pp, X, res, Jc, Jp,
+                                                                      radial);
+  NERO_LAUNCH_CHECK();
+  return NERO_OK;
+}
+
+int nero_sfm_radial_ba_points(const long long* pt_off, int P, const double* res, const double* Jc, const double* Jp, double lambda,
+                              int fix_points, double* Vinv, double* gp, double* Y, void* stream) {
+  if (P < 0 || !(lambda >= 0.0) || (P > 0 && (!pt_off || !res || !Jc || !Jp || !Vinv || !gp || !Y))) return NERO_ERR_ARG;
+  if (P == 0) return NERO_OK;
+  points_kernel<2><<<blocks(P), kBlock, 0, (cudaStream_t)stream>>>(pt_off, P, res, Jc, Jp, lambda, fix_points, Vinv, gp, Y);
+  NERO_LAUNCH_CHECK();
+  return NERO_OK;
+}
+
+int nero_sfm_radial_ba_reduce(const int* ent, const long long* chunk, const int* chunk_key, int nchunk, const long long* seg_chunk,
+                              const int* seg_key, int nseg, const int* obs_seg, const long long* rchunk, const int* rchunk_blk, int nrchunk,
+                              const long long* rseg_chunk, const int* rseg_blk, int nrseg, const int* obs_pt, const int* img_cam, int nimg,
+                              int ncam, const double* Jc, const double* Jp, const double* res, const double* Y, const double* gp,
+                              double lambda, const unsigned char* fixed, double* partial, double* rpartial, double* S, double* b,
+                              void* stream) {
+  return reduce<2>(ent, chunk, chunk_key, nchunk, seg_chunk, seg_key, nseg, obs_seg, rchunk, rchunk_blk, nrchunk, rseg_chunk, rseg_blk, nrseg,
+                   obs_pt, img_cam, nimg, ncam, Jc, Jp, res, Y, gp, lambda, fixed, partial, rpartial, S, b, stream);
+}
+
+int nero_sfm_radial_ba_backsub(const long long* pt_off, int P, const int* obs_img, const int* img_cam, int nimg, int ncam, const double* Jc,
+                               const double* Jp, const double* Vinv, const double* gp, const double* dc, const double* pose,
+                               const double* focal, const double* radial, const double* X, double* pose_new, double* focal_new,
+                               double* radial_new, double* X_new, void* stream) {
+  if (P < 0 || nimg < 1 || ncam < 1 || !dc || !pose || !focal || !radial || !pose_new || !focal_new || !radial_new || !img_cam ||
+      (P > 0 && (!pt_off || !obs_img || !Jc || !Jp || !Vinv || !gp || !X || !X_new)))
+    return NERO_ERR_ARG;
+  backsub_kernel<2><<<blocks((long long)P + nimg + ncam), kBlock, 0, (cudaStream_t)stream>>>(pt_off, P, obs_img, img_cam, nimg, ncam, Jc, Jp,
+                                                                                             Vinv, gp, dc, pose, focal, X, pose_new, focal_new,
+                                                                                             X_new, radial, radial_new);
+  NERO_LAUNCH_CHECK();
+  return NERO_OK;
+}
+
+int nero_sfm_radial_ba_cost(const long long* pt_off, int P, const int* obs_img, const double* obs_xy, const double* pose, const int* img_cam,
+                            const double* focal, const double* pp, const double* radial, const double* X, double* partial, double* cost,
+                            void* stream) {
+  if (P < 1 || !pt_off || !obs_img || !obs_xy || !pose || !img_cam || !focal || !pp || !radial || !X || !partial || !cost) return NERO_ERR_ARG;
+  const cudaStream_t s = (cudaStream_t)stream;
+  const unsigned nb = blocks(P);
+  cost_kernel<2><<<nb, kBlock, 0, s>>>(pt_off, P, obs_img, obs_xy, pose, img_cam, focal, pp, X, partial, radial);
   cost_sum_kernel<<<1, 1, 0, s>>>(partial, (int)nb, cost);
   NERO_LAUNCH_CHECK();
   return NERO_OK;

@@ -26,6 +26,7 @@ _MCSPARSE_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_mcspars
 _MVS_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_mvs.h')  # same library, plain-argument entry points
 _FEATURES_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_features.h')  # same library, plain-argument entry points
 _SFM_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_sfm.h')  # same library, plain-argument entry points
+_SFM_RADIAL_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_sfm_radial.h')  # same library, plain-argument entry points
 _SIMPLIFY_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_simplify.h')  # same library, plain-argument entry points
 _DENOISE_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_denoise.h')  # same library, plain-argument entry points
 _NORMALMAP_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_normalmap.h')  # same library, plain-argument entry points
@@ -126,6 +127,7 @@ MCSPARSE_PROTOS = _parse_header(_MCSPARSE_HEADER)[1]
 MVS_PROTOS = _parse_header(_MVS_HEADER)[1]
 FEATURES_PROTOS = _parse_header(_FEATURES_HEADER)[1]
 SFM_PROTOS = _parse_header(_SFM_HEADER)[1]
+SFM_RADIAL_PROTOS = _parse_header(_SFM_RADIAL_HEADER)[1]
 SIMPLIFY_PROTOS = _parse_header(_SIMPLIFY_HEADER)[1]
 DENOISE_PROTOS = _parse_header(_DENOISE_HEADER)[1]
 NORMALMAP_PROTOS = _parse_header(_NORMALMAP_HEADER)[1]
@@ -135,7 +137,8 @@ UNDISTORT_PROTOS = _parse_header(_UNDISTORT_HEADER)[1]
 for _name, _argtypes in (list(_PROTOS.items()) + list(TEXMAP_PROTOS.items()) + list(ENVMAP_PROTOS.items()) +
                          list(METRICS_PROTOS.items()) + list(RELIGHT_TEX_PROTOS.items()) + list(MESHPTS_PROTOS.items()) +
                          list(OBJPREP_PROTOS.items()) + list(MCSPARSE_PROTOS.items()) + list(MVS_PROTOS.items()) +
-                         list(FEATURES_PROTOS.items()) + list(SFM_PROTOS.items()) + list(SIMPLIFY_PROTOS.items()) +
+                         list(FEATURES_PROTOS.items()) + list(SFM_PROTOS.items()) + list(SFM_RADIAL_PROTOS.items()) +
+                         list(SIMPLIFY_PROTOS.items()) +
                          list(DENOISE_PROTOS.items()) + list(NORMALMAP_PROTOS.items()) + list(GLTF_PROTOS.items()) +
                          list(OCCLUSION_PROTOS.items()) + list(UNDISTORT_PROTOS.items())):
     _fn = getattr(lib, _name)

@@ -9,7 +9,8 @@ COLMAP's incremental scheme in spirit and is not pinned to COLMAP's (DESIGN.md s
 
 The protocol (k_sfm.cu, include/nero_sfm.h):
   * Input.  Cameras, images, keypoints and two_view_geometries of the database (sqlite3); only the stored inlier matches
-    of verified pairs (rows > 0) are used.  Every camera must be SIMPLE_PINHOLE, the model features.py writes.  Camera
+    of verified pairs (rows > 0) are used.  Every camera must have the camera model the mapper estimates: SIMPLE_PINHOLE
+    (the default, what features.py writes by default) or SIMPLE_RADIAL (camera_model='SIMPLE_RADIAL').  Camera
     ids, image ids and names carry through to the model.  The images of the largest connected component of the verified
     pair graph (most images, ties to the lower smallest id) are reconstructed, at most MAX_IMAGES of them; the others are
     reported as not registered.
@@ -43,10 +44,21 @@ The protocol (k_sfm.cu, include/nero_sfm.h):
     segment of an (o, o') list sorted once per adjustment, block partials in block order.
   * Filter.  After every adjustment observations reprojecting beyond MAX_REPROJ px are dropped, then points with fewer
     than two observations or a largest ray angle < MIN_TRI_ANGLE.
-  * Model.  One model of the registered images: SIMPLE_PINHOLE (f, cx, cy) per camera, every keypoint of an image as a
-    POINTS2D entry (point3D id -1 without a point), points numbered 1.. in track order, RGB the rounded mean of the pixels
-    (mvs.read_rgb, stored order) under its observations, error the mean reprojection error of its track.  The same input
-    gives the same bytes.
+  * SIMPLE_RADIAL (include/nero_sfm_radial.h).  Each camera has two free parameters, f and k; the principal point stays
+    fixed.  k starts at the database's value (0 from features.py) and follows the focal's rule: held during the initial
+    pair and while fewer than FOCAL_MIN_IMAGES images are registered, free after that in the registration refinement and
+    in every global adjustment.  Every reprojection error compared with a pixel threshold is measured in the distorted
+    image, where the keypoints are: the adjustment's cost, the filter, a new track's acceptance, track continuation and
+    the model's per-point error.  P3P and the DLT work on rays, so they take the keypoints undistorted with the camera's
+    current (f, k) (undistort.points) as pinhole pixels f x + (cx, cy) of the same camera; a keypoint that is invalid at
+    the current k is left out of that registration or triangulation.  P3P's inlier threshold ABS_POSE_MAX_ERROR is
+    therefore in undistorted pixels.  A DLT point is judged by the distorted reprojection (nero_sfm_radial_filter), not
+    by the DLT's own pixel statistic.  After an adjustment the undistorted keypoints of the cameras whose (f, k) it
+    changed are recomputed.
+  * Model.  One model of the registered images: SIMPLE_PINHOLE (f, cx, cy) or SIMPLE_RADIAL (f, cx, cy, k) per camera,
+    every keypoint of an image as a POINTS2D entry (point3D id -1 without a point), points numbered 1.. in track order,
+    RGB the rounded mean of the pixels (mvs.read_rgb, stored order) under its observations, error the mean reprojection
+    error of its track.  The same input gives the same bytes.
 """
 import math
 import os
@@ -77,6 +89,7 @@ FINAL_BA_ITERS = 100
 LAMBDA0 = 1e-4
 BA_TOL = 1e-12                    # relative cost decrease that ends an adjustment
 SEED = 0
+CAMERA_MODELS = ('SIMPLE_PINHOLE', 'SIMPLE_RADIAL')   # what the mapper estimates (map_sparse.py --camera-model)
 
 
 def _torch():
@@ -112,14 +125,23 @@ def read_database(path):
     return dict(cameras=cams, images=images, keypoints=kps, pairs=pairs)
 
 
-def check_database(db):
-    """The refusals that need no GPU: no verified pair, or a camera model other than SIMPLE_PINHOLE."""
-    bad = sorted(c for c, (m, *_r) in db['cameras'].items() if m != Ft.SIMPLE_PINHOLE)
+def check_database(db, camera_model='SIMPLE_PINHOLE'):
+    """The refusals that need no GPU: an unknown camera_model, a camera of another model than camera_model, or no
+    verified pair."""
+    if camera_model not in CAMERA_MODELS:
+        raise ValueError(f'camera model {camera_model!r}: the mapper estimates {" or ".join(CAMERA_MODELS)} cameras')
+    bad = sorted(c for c, (m, *_r) in db['cameras'].items() if m != Ft.CAMERA_MODELS[camera_model])
     if bad:
         name = objprep.CAMERA_MODELS.get(db['cameras'][bad[0]][0], ('unknown',))[0]
-        raise ValueError(f'camera {bad[0]} is {name}: the mapper reconstructs SIMPLE_PINHOLE cameras only (the model '
-                         'match_features.py writes); distortion models are out of its scope (a SIMPLE_RADIAL model '
-                         'from COLMAP\'s mapper is undistorted by tools/undistort_images.py)')
+        if camera_model == 'SIMPLE_PINHOLE':
+            raise ValueError(f'camera {bad[0]} is {name}: the mapper reconstructs SIMPLE_PINHOLE cameras only (the model '
+                             'match_features.py writes by default); for SIMPLE_RADIAL cameras give --camera-model SIMPLE_RADIAL')
+        raise ValueError(f'camera {bad[0]} is {name}: --camera-model SIMPLE_RADIAL estimates SIMPLE_RADIAL cameras only (write '
+                         'the database with match_features.py --camera-model SIMPLE_RADIAL)')
+    if camera_model == 'SIMPLE_RADIAL':
+        bad = sorted(c for c, (_m, _w, _h, p) in db['cameras'].items() if p.shape[0] != 4 or not np.isfinite(p).all())
+        if bad:
+            raise ValueError(f'camera {bad[0]}: SIMPLE_RADIAL needs 4 finite parameters (f, cx, cy, k)')
     if not db['pairs']:
         raise ValueError('the database has no verified image pair (two_view_geometries with inlier matches)')
 
@@ -197,15 +219,19 @@ def triangulate(off, obs_img, obs_xy, pose, img_cam, focal, pp):
     return X[:T].cpu().numpy(), st[:T].cpu().numpy()
 
 
-def reprojection(pt_off, obs_img, obs_xy, pose, img_cam, focal, pp, X):
-    """-> (err [n, 2] = depth, reprojection error px per observation, angle [P] rad per point)."""
+def reprojection(pt_off, obs_img, obs_xy, pose, img_cam, focal, pp, X, radial=None):
+    """-> (err [n, 2] = depth, reprojection error px per observation, angle [P] rad per point).  With radial (k per
+    camera) the error is measured through SIMPLE_RADIAL, in the distorted image."""
     torch = _torch()
     P = pt_off.shape[0] - 1
     err = torch.empty(max(obs_img.shape[0], 1), 2, dtype=torch.float64, device='cuda')
     ang = torch.empty(max(P, 1), dtype=torch.float64, device='cuda')
-    if P:
+    if P and radial is None:
         _ops().K('nero_sfm_filter', _dev(pt_off, np.int64), P, _dev(obs_img, np.int32), _dev(obs_xy, np.float64),
                  *_cams(pose, img_cam, focal, pp), _dev(X, np.float64), err, ang)
+    elif P:
+        _ops().K('nero_sfm_radial_filter', _dev(pt_off, np.int64), P, _dev(obs_img, np.int32), _dev(obs_xy, np.float64),
+                 *_cams(pose, img_cam, focal, pp), _dev(radial, np.float64), _dev(X, np.float64), err, ang)
     return err[:obs_img.shape[0]].cpu().numpy(), ang[:P].cpu().numpy()
 
 
@@ -225,9 +251,11 @@ def _chunks(counts, key):
 
 class Problem:
     """One bundle adjustment on the device: the point-ordered observations, the parameters and the reduced-system layout
-    (the (o, o') entry list sorted by (row block, column block) once)."""
+    (the (o, o') entry list sorted by (row block, column block) once).  radial (k per camera) makes the cameras
+    SIMPLE_RADIAL (include/nero_sfm_radial.h): each camera then has the two columns (f, k), fixed [6 nimg + 2 ncam]; with
+    None the cameras are SIMPLE_PINHOLE and fixed is [6 nimg + ncam]."""
 
-    def __init__(self, pose, focal, pp, img_cam, X, pt_off, obs_img, obs_xy, fixed, fix_points=False):
+    def __init__(self, pose, focal, pp, img_cam, X, pt_off, obs_img, obs_xy, fixed, fix_points=False, radial=None):
         torch = _torch()
         self.nimg, self.ncam, self.P, self.n = pose.shape[0], focal.shape[0], X.shape[0], obs_img.shape[0]
         if self.nimg > MAX_IMAGES:
@@ -239,7 +267,9 @@ class Problem:
         self.obs_xy = _dev(obs_xy, np.float64)
         self.fixed = _dev(fixed, np.uint8)
         self.fix_points = int(bool(fix_points))
-        self.ncol = 6 * self.nimg + self.ncam
+        self.radial = None if radial is None else _dev(radial, np.float64)
+        kc = 1 if radial is None else 2           # columns per camera
+        self.ncol = 6 * self.nimg + kc * self.ncam
         dev = self.X.device
         cnt = self.pt_off[1:] - self.pt_off[:-1]
         obs_pt = torch.repeat_interleave(torch.arange(self.P, device=dev), cnt)
@@ -268,9 +298,9 @@ class Problem:
         self.rchunk, self.rchunk_blk, self.rseg_chunk = _chunks(rcounts, self.rseg_blk)
         f64 = dict(dtype=torch.float64, device=dev)
         self.res = torch.empty(self.n, 2, **f64)
-        self.Jc = torch.empty(self.n, 2, 7, **f64)
+        self.Jc = torch.empty(self.n, 2, 6 + kc, **f64)
         self.Jp = torch.empty(self.n, 2, 3, **f64)
-        self.Y = torch.empty(self.n, 7, 3, **f64)
+        self.Y = torch.empty(self.n, 6 + kc, 3, **f64)
         self.Vinv = torch.empty(self.P, 9, **f64)
         self.gp = torch.empty(self.P, 3, **f64)
         self.partial = torch.empty(-(-self.P // 256), **f64)
@@ -278,42 +308,58 @@ class Problem:
         self.spartial = torch.empty(max(self.chunk.shape[0], 1), 36, **f64)
         self.bpartial = torch.empty(max(self.rchunk.shape[0], 1), 6, **f64)
 
-    def cost(self, pose=None, focal=None, X=None):
+    def cost(self, pose=None, focal=None, X=None, radial=None):
         ops = _ops()
-        ops.K('nero_sfm_ba_cost', self.pt_off, self.P, self.obs_img, self.obs_xy, self.pose if pose is None else pose, self.img_cam,
-              self.focal if focal is None else focal, self.pp, self.X if X is None else X, self.partial, self.cost_buf, launches=2)
+        pose, focal, X = self.pose if pose is None else pose, self.focal if focal is None else focal, self.X if X is None else X
+        if self.radial is None:
+            ops.K('nero_sfm_ba_cost', self.pt_off, self.P, self.obs_img, self.obs_xy, pose, self.img_cam, focal, self.pp, X, self.partial,
+                  self.cost_buf, launches=2)
+        else:
+            ops.K('nero_sfm_radial_ba_cost', self.pt_off, self.P, self.obs_img, self.obs_xy, pose, self.img_cam, focal, self.pp,
+                  self.radial if radial is None else radial, X, self.partial, self.cost_buf, launches=2)
         return float(self.cost_buf.item())
 
     def linearize(self):
-        _ops().K('nero_sfm_ba_linearize', self.pt_off, self.P, self.obs_img, self.obs_xy, self.pose, self.img_cam, self.focal, self.pp,
-                 self.X, self.res, self.Jc, self.Jp)
+        if self.radial is None:
+            _ops().K('nero_sfm_ba_linearize', self.pt_off, self.P, self.obs_img, self.obs_xy, self.pose, self.img_cam, self.focal, self.pp,
+                     self.X, self.res, self.Jc, self.Jp)
+        else:
+            _ops().K('nero_sfm_radial_ba_linearize', self.pt_off, self.P, self.obs_img, self.obs_xy, self.pose, self.img_cam, self.focal,
+                     self.pp, self.radial, self.X, self.res, self.Jc, self.Jp)
 
     def eliminate(self, lam):
-        _ops().K('nero_sfm_ba_points', self.pt_off, self.P, self.res, self.Jc, self.Jp, float(lam), self.fix_points, self.Vinv, self.gp, self.Y)
+        _ops().K('nero_sfm_ba_points' if self.radial is None else 'nero_sfm_radial_ba_points', self.pt_off, self.P, self.res, self.Jc,
+                 self.Jp, float(lam), self.fix_points, self.Vinv, self.gp, self.Y)
 
     def reduce(self, lam):
         torch = _torch()
         S = torch.zeros(self.ncol, self.ncol, dtype=torch.float64, device='cuda')
         b = torch.zeros(self.ncol, dtype=torch.float64, device='cuda')
-        _ops().K('nero_sfm_ba_reduce', self.ent, self.chunk, self.chunk_key, self.chunk.shape[0], self.seg_chunk, self.seg_key,
-                 self.seg_key.shape[0], self.obs_seg, self.rchunk, self.rchunk_blk, self.rchunk.shape[0], self.rseg_chunk, self.rseg_blk,
-                 self.rseg_blk.shape[0], self.obs_pt, self.img_cam, self.nimg, self.ncam, self.Jc, self.Jp, self.res, self.Y, self.gp,
+        _ops().K('nero_sfm_ba_reduce' if self.radial is None else 'nero_sfm_radial_ba_reduce', self.ent, self.chunk, self.chunk_key,
+                 self.chunk.shape[0], self.seg_chunk, self.seg_key, self.seg_key.shape[0], self.obs_seg, self.rchunk, self.rchunk_blk,
+                 self.rchunk.shape[0], self.rseg_chunk, self.rseg_blk, self.rseg_blk.shape[0], self.obs_pt, self.img_cam, self.nimg, self.ncam, self.Jc, self.Jp, self.res, self.Y, self.gp,
                  float(lam), self.fixed, self.spartial, self.bpartial, S, b, launches=4)
         d = S.diagonal()
         d.copy_(torch.where(d == 0, torch.ones_like(d), d))       # a parameter no observation reaches stays put
         return S, b
 
     def backsub(self, dc):
+        """-> candidate (pose, focal, X), and radial after them for SIMPLE_RADIAL cameras."""
         torch = _torch()
         pose = torch.empty_like(self.pose)
         focal = torch.empty_like(self.focal)
         X = torch.empty_like(self.X)
-        _ops().K('nero_sfm_ba_backsub', self.pt_off, self.P, self.obs_img, self.img_cam, self.nimg, self.ncam, self.Jc, self.Jp, self.Vinv,
-                 self.gp, dc.contiguous(), self.pose, self.focal, self.X, pose, focal, X)
-        return pose, focal, X
+        if self.radial is None:
+            _ops().K('nero_sfm_ba_backsub', self.pt_off, self.P, self.obs_img, self.img_cam, self.nimg, self.ncam, self.Jc, self.Jp, self.Vinv,
+                     self.gp, dc.contiguous(), self.pose, self.focal, self.X, pose, focal, X)
+            return pose, focal, X
+        radial = torch.empty_like(self.radial)
+        _ops().K('nero_sfm_radial_ba_backsub', self.pt_off, self.P, self.obs_img, self.img_cam, self.nimg, self.ncam, self.Jc, self.Jp,
+                 self.Vinv, self.gp, dc.contiguous(), self.pose, self.focal, self.radial, self.X, pose, focal, radial, X)
+        return pose, focal, X, radial
 
     def step(self, lam):
-        """One damped step from the current linearisation -> (candidate pose, focal, X) or None when S is not positive
+        """One damped step from the current linearisation -> the candidate of backsub or None when S is not positive
         definite."""
         torch = _torch()
         self.eliminate(lam)
@@ -335,7 +381,9 @@ class Problem:
                 cand = self.step(lam)
                 new = self.cost(*cand) if cand is not None else math.inf
                 if new < cost:
-                    self.pose, self.focal, self.X = cand
+                    self.pose, self.focal, self.X = cand[:3]
+                    if self.radial is not None:
+                        self.radial = cand[3]
                     lam = max(lam / 10, 1e-12)
                     acc += 1
                     break
@@ -395,7 +443,7 @@ def essential_poses(E):
 class Mapper:
     """The state of one reconstruction: tracks, registered images, points."""
 
-    def __init__(self, db, log=None):
+    def __init__(self, db, log=None, camera_model='SIMPLE_PINHOLE'):
         self.log = log or (lambda s: None)
         self.times = dict(tracks=0.0, init=0.0, register=0.0, triangulate=0.0, bundle=0.0)
         self.db = db
@@ -410,9 +458,14 @@ class Mapper:
         self.img_cam = np.array([cslot[db['images'][i][1]] for i in self.ids], np.int64)
         self.focal = np.array([db['cameras'][c][3][0] for c in self.cam_ids], np.float64)
         self.pp = np.array([db['cameras'][c][3][1:3] for c in self.cam_ids], np.float64)
+        # k per camera for SIMPLE_RADIAL, None for the pinhole mapper
+        self.radial = np.array([db['cameras'][c][3][3] for c in self.cam_ids], np.float64) if camera_model == 'SIMPLE_RADIAL' else None
         self.pairs = {(a, b): v for (a, b), v in db['pairs'].items() if a in slot and b in slot}
         t0 = time.time()
         self._tracks()
+        self.node_und = self.node_xy if self.radial is None else self.node_xy.copy()
+        self.node_ok = np.ones(self.N, bool)
+        self._undistort(np.arange(len(self.cam_ids)))
         self.times['tracks'] = time.time() - t0
         self.pose = np.zeros((n_img, 12))
         self.reg = np.zeros(n_img, bool)
@@ -467,6 +520,27 @@ class Mapper:
     def _track_nodes(self, t):
         return self.tnodes[self.toff[t]:self.toff[t + 1]]
 
+    # -------------------------------------------------------------------------------------------- camera model
+    def _undistort(self, cams):
+        """SIMPLE_RADIAL: the keypoints of cameras `cams` undistorted with their current (f, k) into pinhole pixels
+        f x + (cx, cy) (node_und), and whether each is invertible (node_ok).  P3P and the DLT take these; the pinhole
+        mapper gives them the keypoints as they are."""
+        if self.radial is None:
+            return
+        from . import undistort
+        node_cam = self.img_cam[self.node_img]
+        for c in cams:
+            sel = np.nonzero(node_cam == c)[0]
+            if sel.shape[0]:
+                xn, ok = undistort.points(self.node_xy[sel], self.focal[c], self.pp[c, 0], self.pp[c, 1], self.radial[c])
+                self.node_und[sel] = self.focal[c] * xn.cpu().numpy() + self.pp[c]
+                self.node_ok[sel] = ok.cpu().numpy()
+
+    def _reprojection(self, off, nodes, X):
+        """(depth, reprojection error px) of the nodes and the largest ray angle of each point, measured through the camera
+        model in the image the keypoints come from."""
+        return reprojection(off, self.node_img[nodes], self.node_xy[nodes], self.pose, self.img_cam, self.focal, self.pp, X, self.radial)
+
     # -------------------------------------------------------------------------------------------- helpers
     def _obs_lists(self, tracks, nodes_of):
         """(off [T + 1], nodes) of the given tracks with nodes_of(t) -> their selected nodes."""
@@ -500,15 +574,16 @@ class Mapper:
         cslot = np.full(self.focal.shape[0], -1, np.int64)
         cslot[cams] = np.arange(cams.shape[0])
         nimg, ncam = imgs.shape[0], cams.shape[0]
-        fixed = np.zeros(6 * nimg + ncam, np.uint8)
+        fixed = np.zeros(6 * nimg + (1 if self.radial is None else 2) * ncam, np.uint8)
         if images is None:
             g0, g1 = self.order[0], self.order[1]
             fixed[6 * islot[g0]:6 * islot[g0] + 6] = 1
             fixed[6 * islot[g1] + 3 + int(np.argmax(np.abs(self.pose[g1, 9:])))] = 1
         if self.reg.sum() < FOCAL_MIN_IMAGES:
-            fixed[6 * nimg:] = 1
+            fixed[6 * nimg:] = 1                                  # the focal, and k of SIMPLE_RADIAL
         pr = Problem(self.pose[imgs], self.focal[cams], self.pp[cams], cslot[self.img_cam[imgs]], self.Xt[tracks], off,
-                     islot[self.node_img[nodes]], self.node_xy[nodes], fixed, fix_points)
+                     islot[self.node_img[nodes]], self.node_xy[nodes], fixed, fix_points,
+                     None if self.radial is None else self.radial[cams])
         return pr, imgs, cams, tracks
 
     def _bundle(self, iterations, images=None, fix_points=False, nodes_pt=None):
@@ -524,7 +599,13 @@ class Mapper:
         for k in range(nimg):
             pose[k, :9] = _orthonormal(pose[k, :9].reshape(3, 3)).reshape(-1)
         self.pose[imgs] = pose
+        if self.radial is not None:
+            k = pr.radial.cpu().numpy()
+            changed = cams[(focal != self.focal[cams]) | (k != self.radial[cams])]
+            self.radial[cams] = k
         self.focal[cams] = focal
+        if self.radial is not None:
+            self._undistort(changed)
         if not fix_points:
             self.Xt[tracks] = X
         self.times['bundle'] += time.time() - t0
@@ -537,24 +618,28 @@ class Mapper:
         tracks, off, nodes = self._points()
         if nodes.shape[0] == 0:
             return
-        err, _ = reprojection(off, self.node_img[nodes], self.node_xy[nodes], self.pose, self.img_cam, self.focal, self.pp, self.Xt[tracks])
+        err, _ = self._reprojection(off, nodes, self.Xt[tracks])
         bad = (err[:, 0] <= 0) | (err[:, 1] > MAX_REPROJ)
         self.active[nodes[bad]] = False
         tracks, off, nodes = self._points()
-        _, ang = reprojection(off, self.node_img[nodes], self.node_xy[nodes], self.pose, self.img_cam, self.focal, self.pp, self.Xt[tracks])
+        _, ang = self._reprojection(off, nodes, self.Xt[tracks])
         drop = (np.diff(off) < 2) | (ang < math.radians(MIN_TRI_ANGLE))
         for t in tracks[drop]:
             self.has_pt[t] = False
             self.active[self._track_nodes(t)] = False
 
     def _triangulate(self, tracks, min_angle=MIN_TRI_ANGLE, max_err=MAX_REPROJ):
-        """Triangulate the tracks from their registered observations; keep the good ones.  -> number kept."""
+        """Triangulate the tracks from their registered observations (SIMPLE_RADIAL: the invertible ones, undistorted);
+        keep the good ones.  -> number kept."""
         t0 = time.time()
         tracks = [t for t in tracks if not self.has_pt[t]]
-        sel = lambda t: (lambda nd: nd[self.reg[self.node_img[nd]]])(self._track_nodes(t))
+        sel = lambda t: (lambda nd: nd[self.reg[self.node_img[nd]] & self.node_ok[nd]])(self._track_nodes(t))
         tracks = [t for t in tracks if sel(t).shape[0] >= 2]
         off, nodes = self._obs_lists(tracks, sel)
-        X, st = triangulate(off, self.node_img[nodes], self.node_xy[nodes], self.pose, self.img_cam, self.focal, self.pp)
+        X, st = triangulate(off, self.node_img[nodes], self.node_und[nodes], self.pose, self.img_cam, self.focal, self.pp)
+        if self.radial is not None and tracks:        # judged in the distorted image, not by the DLT's pinhole pixels
+            err, ang = self._reprojection(off, nodes, X)
+            st = np.stack([np.minimum.reduceat(err[:, 0], off[:-1]), np.maximum.reduceat(err[:, 1], off[:-1]), ang], 1)
         ok = (st[:, 0] > 0) & (st[:, 1] <= max_err) & (st[:, 2] >= math.radians(min_angle)) & np.isfinite(X).all(1)
         for k in np.nonzero(ok)[0]:
             t = tracks[k]
@@ -593,13 +678,15 @@ class Mapper:
             self._reset()
             self.reg[[i, j]] = True
             self.order = [i, j]
-            sel = lambda t: (lambda nd: nd[(self.node_img[nd] == i) | (self.node_img[nd] == j)])(self._track_nodes(t))
+            sel = lambda t: (lambda nd: nd[((self.node_img[nd] == i) | (self.node_img[nd] == j)) & self.node_ok[nd]])(self._track_nodes(t))
+            if self.radial is not None:
+                common = np.asarray([t for t in common if sel(t).shape[0] == 2], np.int64)
             off, nodes = self._obs_lists(common, sel)
             best = None
             for R, t in essential_poses(E):
                 self.pose[i] = np.concatenate([np.eye(3).reshape(-1), np.zeros(3)])
                 self.pose[j] = np.concatenate([R.reshape(-1), t])
-                _, st = triangulate(off, self.node_img[nodes], self.node_xy[nodes], self.pose, self.img_cam, self.focal, self.pp)
+                _, st = triangulate(off, self.node_img[nodes], self.node_und[nodes], self.pose, self.img_cam, self.focal, self.pp)
                 front = int((st[:, 0] > 0).sum())
                 if best is None or front > best[0]:
                     best = (front, R, t)
@@ -608,7 +695,7 @@ class Mapper:
             self._bundle(INIT_BA_ITERS)
             self._filter()
             tracks, off, nodes = self._points()
-            ang = reprojection(off, self.node_img[nodes], self.node_xy[nodes], self.pose, self.img_cam, self.focal, self.pp, self.Xt[tracks])[1]
+            ang = self._reprojection(off, nodes, self.Xt[tracks])[1]
             med = math.degrees(float(np.median(ang))) if ang.shape[0] else 0.0
             self.log(f'initial pair {a}, {b}: {self.pairs[a, b][0].shape[0]} inliers, {n0} triangulated, {tracks.shape[0]} points after '
                      f'the two-view adjustment, median angle {med:.1f} deg')
@@ -622,7 +709,7 @@ class Mapper:
     # -------------------------------------------------------------------------------------------- registration
     def _correspondences(self, i):
         nd, t = self._tracks_of_image(i)
-        ok = self.has_pt[t]
+        ok = self.has_pt[t] & self.node_ok[nd]
         return nd[ok], t[ok]
 
     def register(self, i):
@@ -634,7 +721,7 @@ class Mapper:
             self.times['register'] += time.time() - t0
             return False, 0, n
         c = self.img_cam[i]
-        pose, _, cnt, inl, _ = p3p_ransac(self.node_xy[nd], self.Xt[t], self.focal[c], self.pp[c, 0], self.pp[c, 1], self.ids[i])
+        pose, _, cnt, inl, _ = p3p_ransac(self.node_und[nd], self.Xt[t], self.focal[c], self.pp[c, 0], self.pp[c, 1], self.ids[i])
         if cnt < ABS_POSE_MIN_INLIERS or cnt < ABS_POSE_MIN_RATIO * n:
             self.times['register'] += time.time() - t0
             return False, cnt, n
@@ -658,7 +745,7 @@ class Mapper:
         if hp.any():
             nd1, t1 = nd[hp], t[hp]
             off = np.arange(nd1.shape[0] + 1, dtype=np.int64)
-            err, _ = reprojection(off, self.node_img[nd1], self.node_xy[nd1], self.pose, self.img_cam, self.focal, self.pp, self.Xt[t1])
+            err, _ = self._reprojection(off, nd1, self.Xt[t1])
             good = (err[:, 0] > 0) & (err[:, 1] <= MAX_REPROJ)
             self.active[nd1[good]] = True
             cont = int(good.sum())
@@ -696,17 +783,27 @@ class Mapper:
 
     # -------------------------------------------------------------------------------------------- model
     def model(self, image_dir=None):
-        """(cameras, images, points, summary) of the reconstruction in the form objprep.write_colmap_model takes."""
-        from . import mvs
+        """(cameras, images, points, summary) of the reconstruction in the form objprep.write_colmap_model takes.  A
+        SIMPLE_RADIAL camera that undistort.camera would refuse is still written; its message goes to summary['warnings']."""
+        from . import mvs, undistort
         db = self.db
         tracks, off, nodes = self._points()
-        err, _ = reprojection(off, self.node_img[nodes], self.node_xy[nodes], self.pose, self.img_cam, self.focal, self.pp, self.Xt[tracks])
+        err, _ = self._reprojection(off, nodes, self.Xt[tracks])
         regs = np.nonzero(self.reg)[0]
         cams = {}
+        warnings = []
         for c in sorted({int(self.img_cam[i]) for i in regs}):
             cid = self.cam_ids[c]
             _, w, h, _ = db['cameras'][cid]
-            cams[cid] = ('SIMPLE_PINHOLE', w, h, [float(self.focal[c]), float(self.pp[c, 0]), float(self.pp[c, 1])])
+            par = [float(self.focal[c]), float(self.pp[c, 0]), float(self.pp[c, 1])]
+            if self.radial is None:
+                cams[cid] = ('SIMPLE_PINHOLE', w, h, par)
+                continue
+            cams[cid] = ('SIMPLE_RADIAL', w, h, par + [float(self.radial[c])])
+            try:
+                undistort.camera(w, h, *cams[cid][3], name=f'camera {cid}')
+            except ValueError as e:                      # the model is still written; undistort_images.py will refuse it
+                warnings.append(str(e))
         pid = np.full(self.T, -1, np.int64)
         pid[tracks] = np.arange(1, tracks.shape[0] + 1)
         rgb_sum = np.zeros((tracks.shape[0], 3), np.int64)
@@ -739,16 +836,18 @@ class Mapper:
                        points=int(tracks.shape[0]), mean_track=float(cnt.mean()) if cnt.shape[0] else 0.0,
                        mean_error=float(err[:, 1].mean()) if err.shape[0] else 0.0,
                        focals={cid: p[3][0] for cid, p in cams.items()}, dropped_tracks=self.dropped, times=dict(self.times))
+        if self.radial is not None:
+            summary.update(radial={cid: p[3][3] for cid, p in cams.items()}, warnings=warnings)
         return cams, images, points, summary
 
 
-def map_sparse(db_path, output, image_dir=None, log=None):
+def map_sparse(db_path, output, image_dir=None, log=None, camera_model='SIMPLE_PINHOLE'):
     """The whole tool: read the database, reconstruct, write <output>/{cameras,images,points3D}.bin.  -> summary."""
     t0 = time.time()
     db = read_database(db_path)
-    check_database(db)
+    check_database(db, camera_model)
     t1 = time.time()
-    mp = Mapper(db, log).run()
+    mp = Mapper(db, log, camera_model).run()
     cams, images, points, summary = mp.model(image_dir)
     t2 = time.time()
     objprep.write_colmap_model(output, cams, images, points)
