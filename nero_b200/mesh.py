@@ -245,20 +245,41 @@ def marching_cubes(volume, isovalue):
     return v.cpu().numpy().astype(np.float64), t.cpu().numpy().astype(np.int64)
 
 
-def write_ply(path, verts, tris):
-    """Binary little-endian PLY: `float x y z` per vertex, `list uchar int vertex_indices` per triangle."""
+def write_ply(path, verts, tris, colors=None, quality=None):
+    """Binary little-endian PLY: `float x y z` per vertex, `list uchar int vertex_indices` per triangle.  Optional per-vertex
+    colors [V,3] uint8 (`uchar red green blue`) and quality [V] (`float quality`, the scalar field MeshLab and CloudCompare
+    show) follow x y z in that order; without them the file is exactly the plain layout."""
     verts = np.ascontiguousarray(verts, '<f4')
     tris = np.asarray(tris)
     if verts.ndim != 2 or verts.shape[1] != 3 or tris.ndim != 2 or tris.shape[1] != 3:
         raise ValueError(f'write_ply needs verts [V,3] and tris [T,3], got {verts.shape} and {tris.shape}')
     if tris.size and (tris.min() < 0 or tris.max() >= verts.shape[0]):
         raise ValueError('write_ply: triangle index out of range')
+    fields, props = [('p', '<f4', (3,))], 'property float x\nproperty float y\nproperty float z\n'
+    if colors is not None:
+        colors = np.asarray(colors)
+        if colors.shape != verts.shape or colors.dtype != np.uint8:
+            raise ValueError(f'write_ply: colors must be uint8 [{verts.shape[0]},3], got {colors.dtype} {colors.shape}')
+        fields.append(('c', 'u1', (3,)))
+        props += 'property uchar red\nproperty uchar green\nproperty uchar blue\n'
+    if quality is not None:
+        quality = np.asarray(quality)
+        if quality.shape != (verts.shape[0],):
+            raise ValueError(f'write_ply: quality must be [{verts.shape[0]}], got {quality.shape}')
+        fields.append(('q', '<f4'))
+        props += 'property float quality\n'
+    vrec = np.empty(verts.shape[0], dtype=fields)
+    vrec['p'] = verts
+    if colors is not None:
+        vrec['c'] = colors
+    if quality is not None:
+        vrec['q'] = quality
     face = np.empty(tris.shape[0], dtype=[('n', 'u1'), ('v', '<i4', (3,))])
     face['n'] = 3
     face['v'] = tris
-    header = (f'ply\nformat binary_little_endian 1.0\nelement vertex {verts.shape[0]}\nproperty float x\nproperty float y\n'
-              f'property float z\nelement face {tris.shape[0]}\nproperty list uchar int vertex_indices\nend_header\n')
+    header = (f'ply\nformat binary_little_endian 1.0\nelement vertex {verts.shape[0]}\n{props}'
+              f'element face {tris.shape[0]}\nproperty list uchar int vertex_indices\nend_header\n')
     with open(path, 'wb') as f:
         f.write(header.encode('ascii'))
-        f.write(verts.tobytes())
+        f.write(vrec.tobytes())
         f.write(face.tobytes())

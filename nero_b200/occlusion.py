@@ -55,17 +55,8 @@ def _check(rays, distance, seed):
 
 
 def _bvh_cuda(verts, tris):
-    import torch
     from . import ops
-    verts = np.ascontiguousarray(verts.cpu().numpy() if isinstance(verts, torch.Tensor) else verts, np.float32)
-    tris = np.ascontiguousarray(tris.cpu().numpy() if isinstance(tris, torch.Tensor) else tris, np.int32)
-    if tris.ndim != 2 or tris.shape[1] != 3 or tris.shape[0] < 1:
-        raise ValueError(f'the occluder mesh needs tris [T,3] with T >= 1, got {tris.shape}')
-    if tris.min() < 0 or tris.max() >= verts.shape[0]:
-        raise ValueError(f'occluder triangle indices outside [0, {verts.shape[0]})')
-    nodes, btri, _ = ops.bvh_build(verts, tris)
-    dev = torch.device('cuda')
-    return torch.from_numpy(nodes).to(dev), torch.from_numpy(btri).to(dev)
+    return ops.bvh_cuda(verts, tris, 'the occluder mesh')[:2]
 
 
 def points_cuda(points, normals, occluder_verts, occluder_tris, rays=RAYS, distance=DISTANCE, seed=0, keys=None, bvh=None):

@@ -33,6 +33,7 @@ _NORMALMAP_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_normal
 _GLTF_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_gltf.h')  # same library, plain-argument entry points
 _OCCLUSION_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_occlusion.h')  # same library, plain-argument entry points
 _UNDISTORT_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_undistort.h')  # same library, plain-argument entry points
+_MESHDIST_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_meshdist.h')  # same library, plain-argument entry points
 
 ACT_NONE, ACT_SOFTPLUS100, ACT_RELU, ACT_SIGMOID, ACT_EXPCLAMP = 0, 1, 2, 3, 4
 EPI_BIAS_ACT, EPI_MUL_DACT, EPI_TANGENT = 0, 1, 2
@@ -134,13 +135,14 @@ NORMALMAP_PROTOS = _parse_header(_NORMALMAP_HEADER)[1]
 GLTF_PROTOS = _parse_header(_GLTF_HEADER)[1]
 OCCLUSION_PROTOS = _parse_header(_OCCLUSION_HEADER)[1]
 UNDISTORT_PROTOS = _parse_header(_UNDISTORT_HEADER)[1]
+MESHDIST_PROTOS = _parse_header(_MESHDIST_HEADER)[1]
 for _name, _argtypes in (list(_PROTOS.items()) + list(TEXMAP_PROTOS.items()) + list(ENVMAP_PROTOS.items()) +
                          list(METRICS_PROTOS.items()) + list(RELIGHT_TEX_PROTOS.items()) + list(MESHPTS_PROTOS.items()) +
                          list(OBJPREP_PROTOS.items()) + list(MCSPARSE_PROTOS.items()) + list(MVS_PROTOS.items()) +
                          list(FEATURES_PROTOS.items()) + list(SFM_PROTOS.items()) + list(SFM_RADIAL_PROTOS.items()) +
                          list(SIMPLIFY_PROTOS.items()) +
                          list(DENOISE_PROTOS.items()) + list(NORMALMAP_PROTOS.items()) + list(GLTF_PROTOS.items()) +
-                         list(OCCLUSION_PROTOS.items()) + list(UNDISTORT_PROTOS.items())):
+                         list(OCCLUSION_PROTOS.items()) + list(UNDISTORT_PROTOS.items()) + list(MESHDIST_PROTOS.items())):
     _fn = getattr(lib, _name)
     _fn.argtypes, _fn.restype = _argtypes, ctypes.c_int
 # nero_abi_sizeof(i) is the size of ABI_RECORDS[i]; a library built from another version of the header would read the
@@ -521,3 +523,17 @@ def bvh_build(verts, tris):
     n = ctypes.c_int(0)
     call('nero_bvh_build_host', verts, verts.shape[0], tris, T, nodes, tri, ids, ctypes.byref(n))
     return nodes[:n.value].copy(), tri, ids
+
+
+def bvh_cuda(verts, tris, what='the mesh'):
+    """bvh_build of a mesh given as numpy arrays or tensors, uploaded to the current CUDA device -> (nodes, tri, tri_ids)
+    CUDA tensors.  `what` names the mesh in the errors."""
+    verts = np.ascontiguousarray(verts.cpu().numpy() if isinstance(verts, torch.Tensor) else verts, np.float32)
+    tris = np.ascontiguousarray(tris.cpu().numpy() if isinstance(tris, torch.Tensor) else tris, np.int32)
+    if tris.ndim != 2 or tris.shape[1] != 3 or tris.shape[0] < 1:
+        raise ValueError(f'{what} needs tris [T,3] with T >= 1, got {tris.shape}')
+    if tris.min() < 0 or tris.max() >= verts.shape[0]:
+        raise ValueError(f'{what}: triangle indices outside [0, {verts.shape[0]})')
+    nodes, tri, ids = bvh_build(verts, tris)
+    dev = torch.device('cuda')
+    return torch.from_numpy(nodes).to(dev), torch.from_numpy(tri).to(dev), torch.from_numpy(ids).to(dev)
