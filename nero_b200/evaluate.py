@@ -166,8 +166,10 @@ def depth_to_points(depth, K, pose, lo=0.0, hi=float('inf')):
 
 
 # ------------------------------------------------------------------------------------------------ voxel down-sampling
-def voxel_down_sample_cuda(pts, voxel=VOXEL):
-    """Open3D's PointCloud.voxel_down_sample in fp64 on a CUDA tensor [n,3] -> CUDA float64 [m,3].
+def voxel_down_sample_cuda(pts, voxel=VOXEL, extra=None):
+    """Open3D's PointCloud.voxel_down_sample in fp64 on a CUDA tensor [n,3] -> CUDA float64 [m,3].  With extra (a CUDA
+    tensor [n,3], e.g. normals): (points, the voxel means of extra in the same grouping and order); the caller renormalises
+    mean normals.
 
     As Open3D: min bound = the cloud's minimum - voxel/2, voxel index floor((p - min bound) / voxel), each output point the
     mean of its voxel's points.  The sums run in input order.  Output order is ascending voxel key (i, j, k), where Open3D's
@@ -180,8 +182,12 @@ def voxel_down_sample_cuda(pts, voxel=VOXEL):
         raise ValueError(f'voxel size must be positive, got {voxel}')
     p = pts.to(torch.float64).reshape(-1, 3).contiguous()
     n = p.shape[0]
+    if extra is not None:
+        e = extra.to(p.device, torch.float64).reshape(-1, 3).contiguous()
+        if e.shape[0] != n:
+            raise ValueError(f'voxel_down_sample: {e.shape[0]} extra rows for {n} points')
     if n == 0:
-        return p.new_zeros(0, 3)
+        return p.new_zeros(0, 3) if extra is None else (p.new_zeros(0, 3), p.new_zeros(0, 3))
     lo, hi = p.amin(0).cpu().numpy(), p.amax(0).cpu().numpy()
     bounds = np.ascontiguousarray(np.concatenate([lo - voxel * 0.5, hi]), np.float64)
     if (np.floor((bounds[3:] - bounds[:3]) / voxel) >= _KEY_LIMIT).any() or not np.isfinite(bounds).all():
@@ -194,7 +200,11 @@ def voxel_down_sample_cuda(pts, voxel=VOXEL):
     m = ends.shape[0]
     out = torch.empty(m, 3, dtype=torch.float64, device=p.device)
     ops.K('nero_voxel_mean', p, order, ends, m, out)
-    return out
+    if extra is None:
+        return out
+    out2 = torch.empty(m, 3, dtype=torch.float64, device=p.device)
+    ops.K('nero_voxel_mean', e, order, ends, m, out2)
+    return out, out2
 
 
 def voxel_down_sample(points, voxel=VOXEL):
@@ -497,6 +507,20 @@ def read_points_ply(path):
     """Vertex positions float64 [n,3] of a PLY file (the point cloud of Open3D's read_point_cloud, or the vertices of
     read_triangle_mesh).  ascii or binary_little_endian; x, y, z float or double; other vertex properties are skipped; the
     vertex element must come first, and later elements (faces) are not read."""
+    return _read_vertex_columns(path, 'xyz')
+
+
+def read_oriented_points_ply(path):
+    """(points float64 [n,3], normals float64 [n,3]) of an oriented cloud: read_points_ply's rules, with nx, ny, nz float or
+    double.  Reads write_points_ply(..., normals), Open3D's oriented clouds and COLMAP's fused.ply (float x y z nx ny nz
+    uchar red green blue)."""
+    a = _read_vertex_columns(path, ('x', 'y', 'z', 'nx', 'ny', 'nz'))
+    return np.ascontiguousarray(a[:, :3]), np.ascontiguousarray(a[:, 3:])
+
+
+def _read_vertex_columns(path, cols):
+    """The vertex properties `cols` (names) of a PLY file as float64 [n, len(cols)]."""
+    cols = list(cols)
     with open(path, 'rb') as f:
         if f.readline().strip() != b'ply':
             raise ValueError(f'{path}: not a PLY file')
@@ -522,27 +546,37 @@ def read_points_ply(path):
             raise ValueError(f'{path}: the first PLY element must be vertex')
         _, n, props = elems[0]
         names = [p[-1] for p in props]
-        if any(c not in names for c in 'xyz'):
-            raise ValueError(f'{path}: vertex element lacks x, y or z')
+        if any(c not in names for c in cols):
+            if cols[:3] == list('xyz') and len(cols) == 3:
+                raise ValueError(f'{path}: vertex element lacks x, y or z')
+            raise ValueError(f'{path}: vertex element lacks one of {", ".join(cols)}')
         if fmt == 'ascii':
             rows = [f.readline().split() for _ in range(n)]
             if any(p[0] == 'list' for p in props):
-                return np.asarray([[float(r[names.index(c)]) for c in 'xyz'] for r in rows], np.float64).reshape(-1, 3)
+                return np.asarray([[float(r[names.index(c)]) for c in cols] for r in rows], np.float64).reshape(-1, len(cols))
             a = np.asarray(rows, np.float64).reshape(n, len(props))
-            return np.ascontiguousarray(a[:, [names.index(c) for c in 'xyz']])
+            return np.ascontiguousarray(a[:, [names.index(c) for c in cols]])
         if any(p[0] == 'list' for p in props):
             raise ValueError(f'{path}: list properties in a binary vertex element are not supported')
         dt = np.dtype([(p[-1], '<' + _PLY_TYPES[p[0]]) for p in props])
         raw = np.frombuffer(f.read(dt.itemsize * n), dtype=dt, count=n)
-        return np.stack([raw[c].astype(np.float64) for c in 'xyz'], -1)
+        return np.stack([raw[c].astype(np.float64) for c in cols], -1)
 
 
-def write_points_ply(path, points):
+def write_points_ply(path, points, normals=None):
     """Binary little-endian PLY with `double x y z` per vertex and no other element, the layout of Open3D's
-    write_point_cloud for a cloud without normals or colours."""
+    write_point_cloud for a cloud without normals or colours; with normals [n,3], `double x y z nx ny nz`, Open3D's layout
+    for an oriented cloud."""
     p = np.ascontiguousarray(points, '<f8').reshape(-1, 3)
+    props = 'property double x\nproperty double y\nproperty double z\n'
+    if normals is not None:
+        nrm = np.ascontiguousarray(normals, '<f8').reshape(-1, 3)
+        if nrm.shape[0] != p.shape[0]:
+            raise ValueError(f'{nrm.shape[0]} normals for {p.shape[0]} points')
+        p = np.ascontiguousarray(np.concatenate([p, nrm], 1))
+        props += 'property double nx\nproperty double ny\nproperty double nz\n'
     header = (f'ply\nformat binary_little_endian 1.0\ncomment Created by nero_b200\nelement vertex {p.shape[0]}\n'
-              'property double x\nproperty double y\nproperty double z\nend_header\n')
+              + props + 'end_header\n')
     with open(path, 'wb') as f:
         f.write(header.encode('ascii'))
         f.write(p.tobytes())

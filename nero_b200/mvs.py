@@ -50,6 +50,10 @@ The protocol (k_mvs.cu, include/nero_mvs.h):
   * Fusion.  evaluate.depth_to_points_cuda unprojects each view's filtered map in fp64 with cx, cy lowered by 1/2 (it
     unprojects at (x, y)), in (view in name order, row, column) order; --voxel optionally thins the cloud with
     evaluate.voxel_down_sample_cuda.
+  * Normals (normals=True).  Each kept pixel's plane normal n (camera frame) rotated to the world frame in fp64, R^T n with
+    R the world -> camera rotation, in the same order as the points.  With --voxel, each voxel's normals are averaged with
+    its points and the mean renormalised (a mean that cancels to zero stays zero).  They point towards the camera that saw
+    the pixel, i.e. out of the surface.
 """
 import os
 
@@ -293,11 +297,12 @@ def centre_K(K):
 
 
 def reconstruct(views, points, tracks, images, max_size=MAX_SIZE, sources=SOURCES, iterations=ITERATIONS, radius=RADIUS, step=STEP,
-                seed=SEED, voxel=None, trace=None, log=None):
+                seed=SEED, voxel=None, trace=None, log=None, normals=False):
     """The dense cloud of a COLMAP model: views, points and tracks from objprep.read_colmap_model(path, tracks=True);
-    images: a callable name -> uint8 RGB [h,w,3].  -> (points CUDA fp64 [n,3], info).  info holds, per view in name order,
-    names, Ks (fp64, scaled), poses, greys, plan (select_sources), planes, cost, depth (filtered), count; and the
-    ints fused (points before --voxel) and views_used.  trace: dict view index -> list, filled by patchmatch."""
+    images: a callable name -> uint8 RGB [h,w,3].  -> (points CUDA fp64 [n,3], info), or with normals=True (points, normals
+    CUDA fp64 [n,3], info).  info holds, per view in name order, names, Ks (fp64, scaled), poses, greys, plan
+    (select_sources), planes, cost, depth (filtered), count; and the ints fused (points before --voxel) and views_used.
+    trace: dict view index -> list, filled by patchmatch."""
     torch = _torch()
     from .evaluate import depth_to_points_cuda, voxel_down_sample_cuda
     if not 1 <= sources <= _MAX_SRC:
@@ -329,20 +334,34 @@ def reconstruct(views, points, tracks, images, max_size=MAX_SIZE, sources=SOURCE
         if trace is not None:
             tr = trace.setdefault(i, [])
         planes[i], cost[i] = patchmatch(greys[i], Ks[i], [greys[j] for j in src], geo, e['range'], i, iterations, radius, step, seed, tr)
-    depth, count, clouds = [None] * n, [None] * n, []
+    depth, count, clouds, nclouds = [None] * n, [None] * n, [], []
     for i in range(n):
         if planes[i] is None:
             continue
         src = [(Ks[j], poses[j], planes[j], cost[j]) for j in plan[i]['sources'] if planes[j] is not None]
         depth[i], count[i] = geometric_filter(Ks[i], poses[i], planes[i], cost[i], src)
         clouds.append(depth_to_points_cuda(depth[i], poses[i].astype(np.float64), centre_K(Ks[i])))
+        if normals:
+            # the kept pixels in row-major order, as depth_to_points_cuda emits them; n^T R = (R^T n)^T
+            d = depth[i].reshape(-1)
+            keep = (d > 0) & torch.isfinite(d)
+            R = torch.from_numpy(poses[i][:, :3].astype(np.float64)).to(d.device)
+            nclouds.append(planes[i].reshape(-1, 4)[keep, 1:4].to(torch.float64) @ R)
     dev = torch.device('cuda')
     cloud = torch.cat(clouds, 0).to(torch.float64) if clouds else torch.zeros(0, 3, dtype=torch.float64, device=dev)
+    nrm = torch.cat(nclouds, 0) if nclouds else torch.zeros(0, 3, dtype=torch.float64, device=dev)
     fused = int(cloud.shape[0])
     if voxel is not None and fused:
-        cloud = voxel_down_sample_cuda(cloud, voxel)
+        if normals:
+            cloud, nrm = voxel_down_sample_cuda(cloud, voxel, nrm)
+            length = torch.linalg.norm(nrm, dim=1, keepdim=True)
+            nrm = torch.where(length > 0, nrm / torch.where(length > 0, length, torch.ones_like(length)), nrm)
+        else:
+            cloud = voxel_down_sample_cuda(cloud, voxel)
     info = dict(names=names, ids=ids, Ks=Ks, poses=poses, greys=greys, score=score, plan=plan, planes=planes, cost=cost, depth=depth,
                 count=count, fused=fused, views_used=sum(p is not None for p in planes))
+    if normals:
+        return cloud, nrm, info
     return cloud, info
 
 

@@ -35,6 +35,7 @@ _OCCLUSION_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_occlus
 _UNDISTORT_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_undistort.h')  # same library, plain-argument entry points
 _MESHDIST_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_meshdist.h')  # same library, plain-argument entry points
 _ALIGN_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_align.h')  # same library, plain-argument entry points
+_POISSON_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'nero_poisson.h')  # same library, plain-argument entry points
 
 ACT_NONE, ACT_SOFTPLUS100, ACT_RELU, ACT_SIGMOID, ACT_EXPCLAMP = 0, 1, 2, 3, 4
 EPI_BIAS_ACT, EPI_MUL_DACT, EPI_TANGENT = 0, 1, 2
@@ -138,6 +139,7 @@ OCCLUSION_PROTOS = _parse_header(_OCCLUSION_HEADER)[1]
 UNDISTORT_PROTOS = _parse_header(_UNDISTORT_HEADER)[1]
 MESHDIST_PROTOS = _parse_header(_MESHDIST_HEADER)[1]
 ALIGN_PROTOS = _parse_header(_ALIGN_HEADER)[1]
+POISSON_PROTOS = _parse_header(_POISSON_HEADER)[1]
 for _name, _argtypes in (list(_PROTOS.items()) + list(TEXMAP_PROTOS.items()) + list(ENVMAP_PROTOS.items()) +
                          list(METRICS_PROTOS.items()) + list(RELIGHT_TEX_PROTOS.items()) + list(MESHPTS_PROTOS.items()) +
                          list(OBJPREP_PROTOS.items()) + list(MCSPARSE_PROTOS.items()) + list(MVS_PROTOS.items()) +
@@ -145,7 +147,7 @@ for _name, _argtypes in (list(_PROTOS.items()) + list(TEXMAP_PROTOS.items()) + l
                          list(SIMPLIFY_PROTOS.items()) +
                          list(DENOISE_PROTOS.items()) + list(NORMALMAP_PROTOS.items()) + list(GLTF_PROTOS.items()) +
                          list(OCCLUSION_PROTOS.items()) + list(UNDISTORT_PROTOS.items()) + list(MESHDIST_PROTOS.items()) +
-                         list(ALIGN_PROTOS.items())):
+                         list(ALIGN_PROTOS.items()) + list(POISSON_PROTOS.items())):
     _fn = getattr(lib, _name)
     _fn.argtypes, _fn.restype = _argtypes, ctypes.c_int
 # nero_abi_sizeof(i) is the size of ABI_RECORDS[i]; a library built from another version of the header would read the

@@ -1,7 +1,7 @@
 """Reconstruct a custom object's dense point cloud on the GPU: <root>/points.ply from a COLMAP sparse model and its images.
 
     python tools/dense_points.py --root data/custom/kettle [--sparse <model dir>] [--images <dir>] [--output <ply>]
-        [--max-size 1600] [--sources 8] [--iterations 8] [--radius 4] [--step 2] [--seed 0] [--voxel V] [--force]
+        [--max-size 1600] [--sources 8] [--iterations 8] [--radius 4] [--step 2] [--seed 0] [--voxel V] [--normals] [--force]
 
 Replaces the dense half of run_colmap.py (image_undistorter, patch_match_stereo, stereo_fusion), which needs a CUDA build
 of COLMAP: PatchMatch stereo per view, a forward-backward geometric filter against the source views, and the surviving
@@ -10,7 +10,10 @@ tools/prepare_custom_object.py finds it there.  The workflow becomes: match_feat
 mapper) -> dense_points.py -> prepare_custom_object.py.  The protocol and its defaults are stated in nero_b200/mvs.py.
 
 --sparse defaults to <root>/colmap/sparse/0, else <root>/sparse/0; --images to <root>/images.  --voxel (COLMAP units)
-thins the cloud to one point per voxel.  Views without enough source views or sparse points are skipped and reported.
+thins the cloud to one point per voxel.  --normals also writes each point's PatchMatch normal in the world frame
+(`double nx ny nz`, averaged and renormalised per voxel with --voxel), the oriented cloud tools/poisson_mesh.py meshes;
+without it the file is the same as before, byte for byte.  Views without enough source views or sparse points are skipped
+and reported.
 
 Mirror-like parts of a glossy object mostly fail photo-consistency (their appearance changes with the viewpoint) and are
 filtered out.  The table and the less reflective parts of the object still carry the crop, the support plane and the
@@ -43,6 +46,7 @@ def parse_args(argv=None):
     parser.add_argument('--step', type=int, default=2, help='matching window sample step in pixels')
     parser.add_argument('--seed', type=int, default=0)
     parser.add_argument('--voxel', type=float, default=None, help='thin the cloud to one point per voxel of this size')
+    parser.add_argument('--normals', action='store_true', help='also write world-frame unit normals (nx ny nz)')
     parser.add_argument('--force', action='store_true', help='overwrite an existing output file')
     flags = parser.parse_args(argv)
     if not os.path.isdir(flags.root):
@@ -84,12 +88,13 @@ def main(argv=None):
     if not views:
         raise SystemExit(f'{flags.sparse}: the model has no images')
     t0 = time.time()
-    cloud, info = mvs.reconstruct(views, pts, tracks, mvs.image_reader(flags.images), flags.max_size, flags.sources, flags.iterations,
-                                  flags.radius, flags.step, flags.seed, flags.voxel, log=print)
+    out = mvs.reconstruct(views, pts, tracks, mvs.image_reader(flags.images), flags.max_size, flags.sources, flags.iterations,
+                          flags.radius, flags.step, flags.seed, flags.voxel, log=print, normals=flags.normals)
+    cloud, normals, info = out if flags.normals else (out[0], None, out[1])
     cloud = cloud.cpu().numpy()
     if info['views_used'] == 0:
         raise SystemExit('no view has enough source views and sparse points: nothing to reconstruct')
-    write_points_ply(flags.output, cloud)
+    write_points_ply(flags.output, cloud, None if normals is None else normals.cpu().numpy())
     kept = [int((d > 0).sum()) for d in info['depth'] if d is not None]
     print(f'{flags.sparse}: {len(views)} views, {info["views_used"]} reconstructed, {pts.shape[0]} sparse points; '
           f'{info["fused"]} fused points ({sum(kept) / max(1, len(kept)):.0f} per view)'
